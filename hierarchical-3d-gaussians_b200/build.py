@@ -15,7 +15,7 @@ COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-
 # files whose results feed integer artefacts are compiled without FMA contraction
 NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu"}
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_forward.cu", "render_backward.cu",
-           "preprocess_backward.cu", "hierarchy.cu", "loss.cu", "l1_loss.cu", "optim.cu", "peer.cu"]
+           "preprocess_backward.cu", "hierarchy.cu", "loss.cu", "l1_loss.cu", "optim.cu", "peer.cu", "metrics.cu"]
 
 
 def _needs_build(src, obj, deps):

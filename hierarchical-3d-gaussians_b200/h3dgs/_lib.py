@@ -23,10 +23,11 @@ EXPORTS = [
     "h3dgs_profile_enable", "h3dgs_profile_reset", "h3dgs_profile_read", "h3dgs_stage_name",
     "h3dgs_l1_ssim_forward", "h3dgs_l1_ssim_backward", "h3dgs_l1_loss_grad", "h3dgs_l1_loss_grad_peer", "h3dgs_step_status", "h3dgs_sparse_adam",
     "h3dgs_peer_flag_bytes", "h3dgs_peer_alloc", "h3dgs_peer_free", "h3dgs_peer_export", "h3dgs_peer_open", "h3dgs_peer_close",
-    "h3dgs_peer_barrier", "h3dgs_peer_barrier_status",
+    "h3dgs_peer_barrier", "h3dgs_peer_barrier_status", "h3dgs_eval_metrics",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
+EVAL_ROW = 6            # H3DGS_EVAL_ROW: psnr, ssim, overflow, rows, D, longest tile list
 
 
 class RasterArgs(C.Structure):
@@ -110,6 +111,10 @@ def bind(l):
         l.h3dgs_peer_barrier_status.argtypes = [C.c_void_p, C.c_void_p]
     l.h3dgs_lod_cut.restype = C.c_int
     l.h3dgs_lod_cut.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_float] + [C.c_void_p] * 10
+    if hasattr(l, "h3dgs_eval_metrics"):         # evaluation metrics (an emulation build has it when it compiles metrics.cu)
+        l.h3dgs_eval_metrics.restype = C.c_int
+        l.h3dgs_eval_metrics.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] + [C.c_void_p] * 3 + \
+            [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     if hasattr(l, "h3dgs_l1_ssim_forward"):      # loss / optimizer kernels (absent from the emulation build)
         l.h3dgs_l1_ssim_forward.restype = C.c_int
         l.h3dgs_l1_ssim_forward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5

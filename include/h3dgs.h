@@ -271,6 +271,25 @@ int h3dgs_l1_loss_grad_peer(int32_t C, int32_t H, int32_t W, const float* img, c
 int h3dgs_step_status(double* loss_sum, double inv_numel, const int32_t* count, int32_t extra_rows, int32_t row_capacity,
                       const uint32_t* scan_info, int32_t reset_loss, double* out, void* stream);
 
+/* ---- evaluation metrics of one frame (csrc/metrics.cu; render_hierarchy.py:82-113 on top of render_post) ----
+ * img [3,H,W] (the raw rasterizer output), gt [3,H,W], exposure [3][4] or NULL, mask [H,W] or NULL.  In this order:
+ *   a = exposure ? sum_k img[k] * exposure[k][c] + exposure[c][3] : img[c]    (image.permute(1,2,0) @ E[:3,:3] + E[:3,3])
+ *   a = clamp(a, 0, 1), b = clamp(gt, 0, 1); both cropped to columns [x0, W) (x0 = W / 2 is train_test_exp, 0 = off);
+ *   out_img [3,H,W-x0] (optional) = a; then a *= mask, b *= mask;
+ *   psnr = mean_c 20 log10(1 / sqrt(SSE_c / (H (W-x0)))), ssim = mean of the SSIM map (11x11 Gaussian window, sigma 1.5,
+ *   zero padding at the border of the cropped frame).
+ * sums: 4 device doubles of scratch (zeroed here).  A single device thread then stores one row of H3DGS_EVAL_ROW doubles
+ * at results + slot * H3DGS_EVAL_ROW, slot = (*counter)++ (device int; a slot >= max_rows is counted but not stored):
+ *   [0] psnr  [1] ssim  [2] overflow (0/1)  [3] rows = *count + extra_rows  [4] D  [5] longest tile list
+ * with the status of a capacity-mode frame: count (device int, NULL = 0) as h3dgs_lod_cut leaves it, scan_info (NULL =
+ * none) as in h3dgs_state_view; overflow = scan_info[2] != 0 or (row_capacity > 0 and rows > row_capacity).
+ * No host synchronisation: a sweep of frames can be enqueued or replayed from a CUDA graph and read back once. */
+#define H3DGS_EVAL_ROW 6
+int h3dgs_eval_metrics(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure, const float* mask,
+                       int32_t x0, float* out_img, double* sums, const int32_t* count, int32_t extra_rows,
+                       int32_t row_capacity, const uint32_t* scan_info, int32_t* counter, double* results,
+                       int32_t max_rows, void* stream);
+
 /* ---- sparse Adam (SURVEY.md 8f-4; replaces scene/OurAdam.py:249-337 as driven by train_single.py:170-178) ----
  * In-place Adam update of the rows listed in relevant[num_relevant] (int64 row indices) of one parameter
  * tensor viewed as [rows, width]; `step` is the 1-based step count of that tensor (the reference
