@@ -235,6 +235,14 @@ extern "C" size_t h3dgs_expand_scratch_bytes(int32_t N) {
     return align_up(tiles * 8 + 8) + 256;          // tile status words + tile counter | the count of h3dgs_expand_to_size
 }
 
+// every path reads `boxes` as float4 (the bulk copy, the plain-load fallback, interpolation_weights_kernel); only
+// `nodes` may be a view at any 4-byte offset
+static bool boxes_misaligned(const float* boxes, const char* who) {
+    if ((((uintptr_t)boxes) & 15) == 0) return false;
+    set_error("%s: boxes must be 16-byte aligned (got %p)", who, (const void*)boxes);
+    return true;
+}
+
 // one launch of the single-pass cut; scratch holds the tile status words and the tile counter
 static int launch_cut(int N, const int32_t* nodes, const float* boxes, float target_size, const float* target_size_dev,
                       const float* viewpoint, int32_t* render_indices, int32_t* parent_indices, int32_t* nodes_for_render_indices,
@@ -264,6 +272,7 @@ extern "C" int h3dgs_expand_to_size(int32_t N, const int32_t* nodes, const float
                                     void* stream)
 {
     if (N <= 0) return 0;
+    if (boxes_misaligned(boxes, "expand_to_size")) return H3DGS_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     const int tiles = (N + kCutTile - 1) / kCutTile;
     int32_t* total = (int32_t*)((uint8_t*)scratch + align_up((size_t)tiles * 8 + 8));
@@ -285,6 +294,7 @@ extern "C" int h3dgs_lod_cut(int32_t N, const int32_t* nodes, const float* boxes
     if (N <= 0) { set_error("lod_cut: empty hierarchy"); return H3DGS_EINVAL; }
     if (!nodes || !boxes || !viewpoint || !render_indices || !parent_indices || !nodes_for_render_indices || !ts ||
         !num_kids || !count || !scratch) { set_error("lod_cut: NULL argument"); return H3DGS_EINVAL; }
+    if (boxes_misaligned(boxes, "lod_cut")) return H3DGS_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope prof(H3DGS_STAGE_LOD_CUT, s);
     // rows after the cut: index -1 = "skip" for the rasterizer (the head is overwritten by the cut)
@@ -298,6 +308,7 @@ extern "C" int h3dgs_get_interpolation_weights(int32_t n, const int32_t* node_in
                                                float, float, float, float* ts, int32_t* num_kids, void* stream)
 {
     if (n <= 0) return H3DGS_OK;
+    if (boxes_misaligned(boxes, "get_interpolation_weights")) return H3DGS_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope prof(H3DGS_STAGE_LOD_WEIGHTS, s);
     interpolation_weights_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, node_indices, target_size, nodes,

@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib, pipeline
-from .graphstep import GraphedStep, _ptr
+from .graphstep import GraphedStep, _check_index_sizing, _ptr
 
 
 def _metrics(L, H, W, image, gt, exposure, mask, x0, out_image, sums, counter, results, stream, count=None, extra_rows=0,
@@ -54,6 +54,7 @@ class GraphedRender(GraphedStep):
         self.dev = dev
         self.N = scene.means3D.shape[0]
         self.N_nodes = scene.nodes.shape[0]
+        _check_index_sizing(self.N_nodes, self.N)
         self.S = scene.skybox_points
         self.P = int(row_capacity) if row_capacity else self.N
         if not (0 < self.P <= self.N):

@@ -45,6 +45,14 @@ def _ptr(t):
     return None if (t is None or t.numel() == 0) else t.data_ptr()
 
 
+def _check_index_sizing(n_nodes, rows):
+    """h3dgs_lod_cut marks all n_nodes entries of render_indices with -1, and Scene sizes that array by Gaussian rows: a
+    hierarchy with more nodes than rows (nodes that hold no Gaussian) would be written past its end."""
+    if n_nodes > rows:
+        raise ValueError(f"the hierarchy has {n_nodes} nodes but only {rows} Gaussian rows: the device LOD cut needs "
+                         "index arrays of one entry per node")
+
+
 class GraphedStep:
     """scene: pipeline.Scene with a hierarchy.  The camera-independent sizes (W, H, tanfov) are fixed per
     instance (launch constants inside the graphs); camera, target and LOD threshold are device-resident
@@ -68,6 +76,7 @@ class GraphedStep:
         N = scene.means3D.shape[0]                     # rows of the parameter arrays (hierarchy + skybox)
         self.N = N
         self.N_nodes = scene.nodes.shape[0]
+        _check_index_sizing(self.N_nodes, N)
         self.S = scene.skybox_points
         self.P = int(row_capacity) if row_capacity else N
         if not (0 < self.P <= N):

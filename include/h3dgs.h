@@ -194,7 +194,8 @@ int h3dgs_state_layout(int32_t P, int32_t W, int32_t H, int64_t num_rendered,
 
 /* ---- hierarchy LOD cut ---- */
 /* nodes: [N,7] int32 {depth,parent,start,count_leafs,count_merged,start_children,count_children};
- * boxes: [N,2,4] float {min.xyz,size ; max.xyz,_}.  viewpoint is a DEVICE pointer here
+ * boxes: [N,2,4] float {min.xyz,size ; max.xyz,_}, 16-byte aligned (read as float4; the three cut entry points
+ * return H3DGS_EINVAL otherwise, before anything is enqueued); nodes needs only int32 alignment.  viewpoint is a DEVICE pointer here
  * (train_post.py:95 passes the cuda camera_center).  Returns the number of rendered
  * Gaussians (>= 0) or a negative error code; synchronises `stream` (the reference API returns a Python int). */
 int h3dgs_expand_to_size(int32_t N, const int32_t* nodes, const float* boxes, float target_size,
