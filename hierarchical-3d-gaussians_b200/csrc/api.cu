@@ -338,8 +338,7 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
         if (rc) return rc;
     }
     if (!(phases & 2)) return H3DGS_OK;
-    static const bool k9_serial = [] { const char* e = getenv("H3DGS_K9_SERIAL"); return e && e[0] == '1'; }();
-    if (!zero_joined && !a->debug && !a->colors_precomp && !k9_serial) {
+    if (!zero_joined && !a->debug && !a->colors_precomp) {
         // scatter mode: every output is an atomic reduction, so the SH kernel (side stream, right
         // after its zero-fill) and the covariance kernel (main stream) run concurrently
         H3_CUDA(cudaEventRecord(ss->fork, s));                           // accum is complete at this point of s
