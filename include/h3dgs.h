@@ -291,6 +291,16 @@ int h3dgs_eval_metrics(int32_t H, int32_t W, const float* img, const float* gt, 
                        int32_t row_capacity, const uint32_t* scan_info, int32_t* counter, double* results,
                        int32_t max_rows, void* stream);
 
+/* ---- exact 3-nearest-neighbour distances (csrc/knn.cu; simple_knn._C.distCUDA2, scene/gaussian_model.py:21, 190-194) ----
+ * points [P,3] float, mean_dist2 [P] float.  mean_dist2[i] = ((b0 + b1) + b2) / 3.0f, where b0 <= b1 <= b2 are the three
+ * smallest d = (dx*dx + dy*dy) + dz*dz, dx = q.x - p.x (fp32, every operation rounded, no FMA), over the points q of OTHER
+ * indices (an exact duplicate of p counts, with d = 0).  A missing neighbour (fewer than three other points) counts as
+ * FLT_MAX.  Points with a non-finite coordinate are ignored by every finite point; their own rows are unspecified.
+ * The result depends only on the set of points.  scratch: >= h3dgs_knn_scratch_bytes(P) device bytes, 256-byte aligned.
+ * No host synchronisation.  P = 0 enqueues nothing; P < 0, or a NULL pointer with P > 0, is H3DGS_EINVAL. */
+size_t h3dgs_knn_scratch_bytes(int64_t P);
+int h3dgs_dist_knn3(int32_t P, const float* points, float* mean_dist2, void* scratch, void* stream);
+
 /* ---- sparse Adam (SURVEY.md 8f-4; replaces scene/OurAdam.py:249-337 as driven by train_single.py:170-178) ----
  * In-place Adam update of the rows listed in relevant[num_relevant] (int64 row indices) of one parameter
  * tensor viewed as [rows, width]; `step` is the 1-based step count of that tensor (the reference
