@@ -147,9 +147,14 @@ __device__ __forceinline__ void group_pixel(int tile_x, int tile_y, int warp, in
     px = tile_x * kTile + 8 * (warp & 1) + 4 * (g & 1) + (k & 3);
     py0 = tile_y * kTile + 8 * (warp >> 1) + 4 * (g >> 1) + 2 * (k >> 2);
 }
-// The group walk is the default (on config #3 it runs 27 % fewer loop iterations than the one-list-per-warp walk, at 2.3x
-// the gradient reductions); H3DGS_GROUPWALK=0 selects the one-list-per-warp variants.
-inline bool use_group_walk() { const char* e = getenv("H3DGS_GROUPWALK"); return !(e && e[0] == '0'); }
+// Each kernel defaults to the walk that is faster for it on the H100 (DESIGN.md §3.1): the backward walks per group (on
+// config #3 it runs 27 % fewer loop iterations than the one-list-per-warp walk, at 2.3x the gradient reductions), the
+// forward walks one list per warp.  H3DGS_GROUPWALK=1 forces the group walk in both kernels, H3DGS_GROUPWALK=0 one list per warp in both; the two walks
+// compute the same results bit for bit.
+inline bool use_group_walk(bool dflt) {
+    const char* e = getenv("H3DGS_GROUPWALK");
+    return (e && e[0]) ? e[0] != '0' : dflt;
+}
 
 #endif
 

@@ -3,7 +3,8 @@
 //
 // Device build (included from common.cuh): sm_90 has no packed FP32 instructions, so a pair is two
 // registers and every operation is two FFMA / FMUL / FADD.  The entry's record, its dx terms and the
-// survivor loop are still shared by the two pixels.  Each lane is an IEEE fma/mul/add.rn.
+// survivor loop are still shared by the two pixels.  Each lane is an IEEE fma/mul/add.rn; only the gradient
+// terms of pair_grad, which decide nothing, are plain float expressions that nvcc may contract.
 //
 // Host build (-DH3_PAIR_HOST_EMU, plain g++): the same functions over a two-float struct, so that the
 // formulas -- exponent, capped alpha, hierarchy weight, the back-to-front gradient recurrence -- can be
@@ -67,7 +68,7 @@ H3_PM_FN float fast_rcp(float x) { const float r = rcp_approx(x); return r * (2.
 H3_PM_FN f2 rcp2(f2 x) {
     float x0, x1; upk(x, x0, x1);
     const f2 r = pk(rcp_approx(x0), rcp_approx(x1));
-    return mul2(r, sub2(bc(2.0f), mul2(x, r)));
+    return mul2(r, fma2(pk(-x0, -x1), r, bc(2.0f)));
 }
 
 // Gaussian exponent of one entry at the thread's two pixels, shared by forward and backward so that
@@ -167,29 +168,38 @@ struct PairState { f2 T, acc; };
 // zero for a pixel that does not take the entry: every term below then is an exact zero (each carries
 // a factor G or alpha, the other factors are finite) and its state is unchanged.
 // cg = colour . dL/dC of the pair, neg_bg_dot = -(background . dL/dC), g0..gd = dL/dC channels.
+// The gradient terms decide nothing, so they are free to contract (FFMA where a product feeds a sum).  dx is shared by the pair, so the five terms of the exponent's gradient need only the three moments
+// S_k = sum_i d_i^k G_i dL/dab_i (k = 0, 1, 2) of the pair, with dL/dG = opacity dL/dab:
+//   v0 = o (-cy S1 - cx dx S0), v1 = o (-cy dx S0 - cz S1), v2 = o dx^2 S0, v3 = o dx S1, v4 = o S2, v5 = S0.
+// v[9] is written only with DEPTH.
 template <bool HIER, bool DEPTH>
 H3_PM_FN void pair_grad(const float4& a, const float4& bb, float dx, f2 d, f2 G, f2 alpha, f2 dadb, f2 cg, f2 T_final,
                         f2 neg_bg_dot, f2 g0, f2 g1, f2 g2, f2 gd, PairState& st, float (&v)[10])
 {
     const f2 rcp = rcp2(sub2(bc(1.0f), alpha));            // one reciprocal serves T and the background term
-    const f2 Tn = mul2(st.T, rcp);
     const f2 diff = sub2(cg, st.acc);
-    const f2 dL_dalpha = fma2(mul2(T_final, rcp), neg_bg_dot, mul2(diff, Tn));
+    // dL/dalpha = (T_final neg_bg_dot + T diff) / (1 - alpha); T_final neg_bg_dot is loop-invariant in the kernels
+    const f2 dL_dalpha = mul2(fma2(st.T, diff, mul2(T_final, neg_bg_dot)), rcp);
     const f2 dL_dab = HIER ? mul2(dL_dalpha, dadb) : dL_dalpha;
-    const f2 w = mul2(alpha, Tn);                          // d(pixel colour)/d(entry colour)
-    st.T = Tn;
+    st.T = mul2(st.T, rcp);
+    const f2 w = mul2(alpha, st.T);                        // d(pixel colour)/d(entry colour)
     st.acc = fma2(alpha, diff, st.acc);
-    const f2 dL_dG = mul2(bc(bb.y), dL_dab);
-    const f2 gdx = mul2(G, bc(dx)), gdy = mul2(G, d);
-    const f2 qx = mul2(gdx, dL_dG), qy = mul2(gdy, dL_dG);
-    v[0] = hsum(fma2(qy, bc(-a.w), mul2(qx, bc(-a.z))));   // dL_dG (-gdx cx - gdy cy)
-    v[1] = hsum(fma2(qx, bc(-a.w), mul2(qy, bc(-bb.x))));  // dL_dG (-gdy cz - gdx cy)
-    v[2] = hsum(qx) * dx;
-    v[3] = hsum(mul2(qx, d));
-    v[4] = hsum(mul2(qy, d));
-    v[5] = hsum(mul2(G, dL_dab));
-    v[6] = hsum(mul2(w, g0)); v[7] = hsum(mul2(w, g1)); v[8] = hsum(mul2(w, g2));
-    v[9] = DEPTH ? hsum(mul2(w, gd)) : 0.f;
+    float p0, p1, d0, d1;
+    upk(mul2(G, dL_dab), p0, p1);
+    upk(d, d0, d1);
+    const float dp0 = d0 * p0, dp1 = d1 * p1;
+    const float S0 = p0 + p1, S1 = dp0 + dp1, S2 = fmaf(d0, dp0, d1 * dp1);
+    const float oS0 = bb.y * S0, oS1 = bb.y * S1, dxoS0 = dx * oS0;
+    v[0] = fmaf(-a.w, oS1, -a.z * dxoS0);
+    v[1] = fmaf(-a.w, dxoS0, -bb.x * oS1);
+    v[2] = dx * dxoS0;
+    v[3] = dx * oS1;
+    v[4] = bb.y * S2;
+    v[5] = S0;
+    float w0, w1;
+    upk(w, w0, w1);
+    v[6] = fmaf(w0, lo(g0), w1 * hi(g0)); v[7] = fmaf(w0, lo(g1), w1 * hi(g1)); v[8] = fmaf(w0, lo(g2), w1 * hi(g2));
+    if (DEPTH) v[9] = fmaf(w0, lo(gd), w1 * hi(gd));
 }
 
 }  // namespace h3dgs

@@ -2,9 +2,10 @@
 // Semantics per oracle/oracle.c::oracle_render_backward.
 //
 // One CTA (128 threads, two pixels each) per tile, records streamed back-to-front with the same TMA
-// double buffer as the forward; the arithmetic of a thread's two pixels is pair_math.cuh's; per-entry partials of a warp's 64 pixels are reduced with a
-// transpose-reduce (12 shuffles for 10 values) and 10 lanes issue ONE red.global.add for the warp --
-// 64x fewer atomics than the classic one-atomic-per-pixel formulation.
+// double buffer as the forward; the arithmetic of a thread's two pixels is pair_math.cuh's; per-entry partials are reduced
+// over the group's 8 lanes (group walk) or the warp (one list per warp) with a transpose-reduce (span_reduce), and the
+// lanes holding the 9 (10 with depth) totals issue one or two predicated red.global.add per entry --
+// 16x to 64x fewer atomics than the classic one-atomic-per-pixel formulation.
 #include "common.cuh"
 #include "tma.cuh"
 
@@ -21,65 +22,36 @@ constexpr int kBwdMinBlocks = 1;
 #endif
 constexpr int kBwdStages = 2;
 
-// Reduce NV per-lane values over the 32 lanes of a warp with a transpose-reduce: at every
-// butterfly level each lane keeps half of its values and ships the other half, so the whole
-// reduction costs 5+3+2+1+1 = 12 shuffles for 10 values instead of 10 x 5 = 50, and the 10
-// totals end up on 10 DIFFERENT lanes -- which then issue ONE predicated red.global.add for
-// the warp (a contiguous 40-B row) instead of 10 serial atomics from lane 0.
-// Returns this lane's total; `slot` (precomputed per lane by reduce_slot) says which value it is.
-__device__ __forceinline__ int reduce_slot(int lane) {
-    if (lane & 1) return -1;
-    const int b4 = (lane >> 4) & 1, b3 = (lane >> 3) & 1, b2 = (lane >> 2) & 1, b1 = (lane >> 1) & 1;
-    int ai;                                  // index within the 5 values kept after level 16
-    if (!b3) { if (b2 && b1) return -1; ai = b2 ? 2 : b1; }
-    else     { if (b2) return -1; ai = 3 + b1; }
-    return 5 * b4 + ai;
-}
+// Reduce the per-lane partials v[0..8] (v[0..9] with DEPTH) over every aligned span of SPAN lanes (8: a group of the
+// group walk, 32: the warp) with a transpose-reduce.  Eight of them, u = v[0..3], v[5..8], go down the span's three top
+// lane bits: at every level each lane keeps half of its values and ships the other half (4 + 2 + 1 shuffles), so the
+// lanes whose top bits read q = 4 b_top + 2 b_mid + b_low end up with the total of u[q] (span_slot); a 32-lane span adds
+// the lower two bits by plain butterflies.  v[4] rides along as a plain butterfly in x; with DEPTH it is paired with v[9]
+// at the top level, so x holds the total of v[9] on the lanes whose top bit is set.  Per span: 10 shuffles (8 lanes) or
+// 14 (32 lanes) and 14 selects (16 with DEPTH) for 9 or 10 values, instead of 10 x 3 or 10 x 5 shuffles.
 __device__ __forceinline__ float xchg_add(float keep, float send, int mask) {
     return keep + __shfl_xor_sync(0xffffffffu, send, mask);
 }
-// two exchanges and their additions, as a pair
-__device__ __forceinline__ f2 xchg_add2(float keep0, float send0, float keep1, float send1, int mask) {
-    return add2(pk(keep0, keep1), pk(__shfl_xor_sync(0xffffffffu, send0, mask), __shfl_xor_sync(0xffffffffu, send1, mask)));
+template <int SPAN, bool DEPTH>
+__device__ __forceinline__ float span_reduce(const float (&v)[10], int lane, float& x) {
+    constexpr int top = SPAN / 2, mid = SPAN / 4, low = SPAN / 8;
+    const bool bt = lane & top, bm = lane & mid, bl = lane & low;
+    float a[4], b[2];
+#pragma unroll
+    for (int i = 0; i < 4; i++) a[i] = xchg_add(bt ? v[5 + i] : v[i], bt ? v[i] : v[5 + i], top);
+    x = DEPTH ? xchg_add(bt ? v[9] : v[4], bt ? v[4] : v[9], top) : xchg_add(v[4], v[4], top);
+#pragma unroll
+    for (int i = 0; i < 2; i++) b[i] = xchg_add(bm ? a[2 + i] : a[i], bm ? a[i] : a[2 + i], mid);
+    x = xchg_add(x, x, mid);
+    float r = xchg_add(bl ? b[1] : b[0], bl ? b[0] : b[1], low);
+    x = xchg_add(x, x, low);
+#pragma unroll
+    for (int m = low / 2; m >= 1; m /= 2) { r = xchg_add(r, r, m); x = xchg_add(x, x, m); }
+    return r;
 }
-__device__ __forceinline__ float transpose_reduce10(const float (&v)[10], int lane) {
-    const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4, b1 = lane & 2;
-    float a[5];
-    upk(xchg_add2(b4 ? v[5] : v[0], b4 ? v[0] : v[5], b4 ? v[6] : v[1], b4 ? v[1] : v[6], 16), a[0], a[1]);
-    upk(xchg_add2(b4 ? v[7] : v[2], b4 ? v[2] : v[7], b4 ? v[8] : v[3], b4 ? v[3] : v[8], 16), a[2], a[3]);
-    a[4] = xchg_add(b4 ? v[9] : v[4], b4 ? v[4] : v[9], 16);
-    // 5 -> (3 | 2)
-    float b[3];
-    upk(xchg_add2(b3 ? a[3] : a[0], b3 ? a[0] : a[3], b3 ? a[4] : a[1], b3 ? a[1] : a[4], 8), b[0], b[1]);
-    b[2] = xchg_add(b3 ? 0.f : a[2], b3 ? a[2] : 0.f, 8);
-    // 3 -> (2 | 1)
-    float c[2];
-    upk(xchg_add2(b2 ? b[2] : b[0], b2 ? b[0] : b[2], b2 ? 0.f : b[1], b2 ? b[1] : 0.f, 4), c[0], c[1]);
-    // 2 -> (1 | 1)
-    float d = xchg_add(b1 ? c[1] : c[0], b1 ? c[0] : c[1], 2);
-    d += __shfl_xor_sync(0xffffffffu, d, 1);
-    return d;
-}
-
-// Group walk: the same reduction over the 8 lanes of a group (xor 4, 2, 1): 5 + 3 + 2 = 10 shuffles leave the 10 totals
-// on 6 of the 8 lanes -- lanes with bit0 = 0 hold two (r0, r1), lanes with bit0 = 1 and bit1 = 0 hold one (r0).
-// group_slots(lane & 7) gives the accum columns of (r0, r1), -1 = none.
-__device__ __forceinline__ void group_slots(int k, int& s0, int& s1) {
-    const int b2 = (k >> 2) & 1, b1 = (k >> 1) & 1, b0 = k & 1, base = 5 * b2;
-    if (!b0) { s0 = base + (b1 ? 3 : 0); s1 = base + (b1 ? 4 : 1); }
-    else { s0 = b1 ? -1 : base + 2; s1 = -1; }
-}
-__device__ __forceinline__ void transpose_reduce10_g8(const float (&v)[10], int lane, float& r0, float& r1) {
-    const bool b2 = lane & 4, b1 = lane & 2, b0 = lane & 1;
-    float a[5];
-    upk(xchg_add2(b2 ? v[5] : v[0], b2 ? v[0] : v[5], b2 ? v[6] : v[1], b2 ? v[1] : v[6], 4), a[0], a[1]);
-    upk(xchg_add2(b2 ? v[7] : v[2], b2 ? v[2] : v[7], b2 ? v[8] : v[3], b2 ? v[3] : v[8], 4), a[2], a[3]);
-    a[4] = xchg_add(b2 ? v[9] : v[4], b2 ? v[4] : v[9], 4);
-    float b[3];
-    upk(xchg_add2(b1 ? a[3] : a[0], b1 ? a[0] : a[3], b1 ? a[4] : a[1], b1 ? a[1] : a[4], 2), b[0], b[1]);
-    b[2] = xchg_add(b1 ? 0.f : a[2], b1 ? a[2] : 0.f, 2);
-    upk(xchg_add2(b0 ? b[2] : b[0], b0 ? b[0] : b[2], b0 ? 0.f : b[1], b0 ? b[1] : 0.f, 1), r0, r1);
-}
+// accum column of span_reduce's r on lane k of its span: u[q] with q = k / (SPAN / 8)
+template <int SPAN>
+__device__ __forceinline__ int span_slot(int k) { const int q = k / (SPAN / 8); return q < 4 ? q : q + 1; }
 
 constexpr int kBwdThreads = 128;      // two vertically adjacent pixels per thread (see render_forward.cu)
 
@@ -99,10 +71,9 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
     __shared__ __align__(128) Record s_rec[kBwdStages][kBwdBatch];
     __shared__ uint32_t s_id[kBwdStages][kBwdBatch];
     __shared__ __align__(8) uint64_t s_full[kBwdStages];
-    __shared__ uint8_t s_list[GROUPS ? kBwdThreads / 32 : 1][4][GROUPS ? kBwdBatch : 4];   // group walk: per warp, four lists of entry positions
+    __shared__ __align__(16) uint8_t s_list[GROUPS ? kBwdThreads / 32 : 1][4][GROUPS ? kBwdBatch : 4];   // group walk: per warp, four lists of entry positions
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int slot = reduce_slot(lane);
     const int tile_x = blockIdx.x % gx;
     const int tile_y = (blockIdx.x / gx) * shard_count + shard_index;
     const int tile = tile_y * gx + tile_x;
@@ -124,6 +95,8 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
         }
     };
     for (int it = 0; it < kBwdStages && it < nb; it++) stage_ids(it);
+    if (GROUPS)                           // the warp's four lists: 4 kBwdBatch bytes = kBwdBatch words
+        for (int k = lane; k < kBwdBatch; k += 32) reinterpret_cast<uint32_t*>(&s_list[warp][0][0])[k] = 0u;
     if (tid == 0) {
         for (int s = 0; s < kBwdStages; s++) mbar_init(&s_full[s], 1);
         fence_mbar_init();
@@ -141,8 +114,12 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
     int px, py0;
     if (GROUPS) group_pixel(tile_x, tile_y, warp, lane, px, py0);
     else quad_pixel(tile_x, tile_y, warp, lane, px, py0);
-    int gs0, gs1;
-    group_slots(lane & 7, gs0, gs1);
+    // accum columns this lane adds (-1: none): group walk, r of span_reduce<8> and x on lane 0 (v[4]) and lane 4 (v[9]);
+    // one list per warp, see the reduction below
+    const int k8 = lane & 7;
+    const int slot = GROUPS ? span_slot<8>(k8)
+                            : (lane & 3) == 0 ? span_slot<32>(lane) : lane == 1 ? 4 : (DEPTH && lane == 17) ? 9 : -1;
+    const int xslot = k8 == 0 ? 4 : (DEPTH && k8 == 4) ? 9 : -1;
     const int grp = lane >> 3;
     const int py1 = py0 + 1;
     const bool in0 = px < W && py0 < H, in1 = px < W && py1 < H;
@@ -214,18 +191,18 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
             if (DEPTH) cg = fma2(bc(c.w), gd, cg);
             float v[10];
             pair_grad<HIER, DEPTH>(a, bb, dx, d, G, al, dadb, cg, Tf, neg_bgd, g0, g1, g2, gd, ps, v);
+            float* row = accum + (size_t)gid * kAccum;
+            float x;
             if (GROUPS) {
                 // every group reduces its own entry over its 8 lanes; groups without a taker stay silent
                 const bool taker = ((__ballot_sync(0xffffffffu, v0 || v1) >> (8 * grp)) & 0xFFu) != 0u;
-                float r0, r1;
-                transpose_reduce10_g8(v, lane, r0, r1);
-                float* row = accum + (size_t)gid * kAccum;
-                if (taker && gs0 >= 0 && (DEPTH || gs0 < 9)) atomicAdd(row + gs0, r0);
-                if (taker && gs1 >= 0 && (DEPTH || gs1 < 9)) atomicAdd(row + gs1, r1);
+                const float r = span_reduce<8, DEPTH>(v, lane, x);
+                if (taker) atomicAdd(row + slot, r);
+                if (taker && xslot >= 0) atomicAdd(row + xslot, x);
             } else {
-                const float total = transpose_reduce10(v, lane);
-                float* row = accum + (size_t)gid * kAccum;
-                if (slot >= 0 && (DEPTH || slot < 9)) atomicAdd(row + slot, total);
+                // lanes 4 q hold the totals of u[q], lane 1 the total of v[4], lane 17 (DEPTH) the one of v[9]: one atomic
+                const float r = span_reduce<32, DEPTH>(v, lane, x);
+                if (slot >= 0) atomicAdd(row + slot, (lane & 3) == 0 ? r : x);
             }
         };
         if (GROUPS) {
@@ -251,10 +228,9 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
             const int mylen = grp == 0 ? c0 : grp == 1 ? c1 : grp == 2 ? c2 : c3;
             const int maxlen = max(max(c0, c1), max(c2, c3));
             const uint8_t* my = lst + grp * kBwdBatch;
-            for (int i = maxlen - 1; i >= 0; i--) {
-                const bool has = i < mylen;
-                replay_entry(has ? (int)my[i] : 0, has);
-            }
+            // positions past a group's own list are stale entries of an earlier list (zeroed at the start), so they name
+            // records of the batch and the load needs no branch; has = false keeps them out of the sums and the state
+            for (int i = maxlen - 1; i >= 0; i--) replay_entry((int)my[i], i < mylen);
             __syncwarp();                     // the lists are rebuilt for the next batch
         } else {
             // back to front; per round of 32 entries a ballot compacts the entries that can reach this warp's quadrant at all
@@ -291,7 +267,7 @@ int launch_render_backward(const h3dgs_raster_args& a, const uint32_t* ranges, c
     const bool depth = a.do_depth != 0 && dL_dinvdepth != nullptr;
     const dim3 grid(gx * rows), block(kBwdThreads);
     ProfScope prof(H3DGS_STAGE_RENDER_BWD, s);
-    const bool groups = use_group_walk();
+    const bool groups = use_group_walk(true);
 #define LAUNCH(HI, DE, GR)                                                                                          \
     render_backward_kernel<HI, DE, GR><<<grid, block, 0, s>>>(W, H, gx, sc, si, (const uint2*)ranges, sorted_records, \
                                                               point_list, a.bg, final_T, n_contrib, tile_max_contrib, \

@@ -232,7 +232,7 @@ int launch_render_forward(const h3dgs_raster_args& a, const uint32_t* ranges, co
     const bool depth = a.do_depth != 0;
     const dim3 grid(gx * rows), block(kFwdThreads);
     ProfScope prof(H3DGS_STAGE_RENDER_FWD, s);
-    const bool groups = use_group_walk();
+    const bool groups = use_group_walk(false);
     const PeerPtrs peers = peer_ptrs(a.peer_image, a.peer_count);
 #define LAUNCH(HI, DE, GR)                                                                                         \
     render_forward_kernel<HI, DE, GR><<<grid, block, 0, s>>>(W, H, gx, sc, si, (const uint2*)ranges, sorted_records, \
