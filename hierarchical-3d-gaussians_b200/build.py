@@ -12,12 +12,12 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",
           "-ccbin", "/usr/bin/g++"]
-# files whose results feed integer artefacts, or whose arithmetic is pinned bit for bit (knn.cu), are compiled
-# without FMA contraction
-NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu", "knn.cu"}
+# files whose results feed integer artefacts, or whose arithmetic is pinned bit for bit (knn.cu, the Morton keys of
+# hier_build.cu), are compiled without FMA contraction
+NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu", "knn.cu", "hier_build.cu"}
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_forward.cu", "render_backward.cu",
            "preprocess_backward.cu", "hierarchy.cu", "loss.cu", "l1_loss.cu", "optim.cu", "peer.cu", "metrics.cu",
-           "knn.cu"]
+           "knn.cu", "hier_build.cu"]
 
 
 def _needs_build(src, obj, deps):

@@ -19,6 +19,7 @@
 #include <float.h>
 #include <math.h>
 #include "common.cuh"
+#include "float_key.cuh"
 
 namespace h3dgs {
 namespace {
@@ -54,23 +55,8 @@ KnnLayout knn_layout(int64_t P) {
     return l;
 }
 
-__device__ __forceinline__ uint32_t f2key(float f) {
-    const uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key2f(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 __device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
-__device__ __forceinline__ float warp_min(float v) {
-    for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(kFull, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(kFull, v, o));
-    return v;
-}
 
 // the pinned distance: dx = q.x - p.x, d = (dx*dx + dy*dy) + dz*dz, every operation rounded
 __device__ __forceinline__ float dist2(float4 q, float px, float py, float pz) {

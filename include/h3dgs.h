@@ -8,6 +8,8 @@
  *   gaussian_hierarchy._C.expand_to_size                        -> h3dgs_expand_to_size
  *   gaussian_hierarchy._C.get_interpolation_weights             -> h3dgs_get_interpolation_weights
  *   (both of the above, device-side, for a graph-captured step)  -> h3dgs_lod_cut
+ *   simple_knn._C.distCUDA2                                      -> h3dgs_dist_knn3
+ *   the GaussianHierarchyCreator executable                      -> h3dgs_build_hierarchy
  *
  * The reference binds those through two pip packages whose source is absent from
  * the reference checkout (empty submodules, .gitmodules:5-13); the interface is pinned by
@@ -300,6 +302,43 @@ int h3dgs_eval_metrics(int32_t H, int32_t W, const float* img, const float* gt, 
  * No host synchronisation.  P = 0 enqueues nothing; P < 0, or a NULL pointer with P > 0, is H3DGS_EINVAL. */
 size_t h3dgs_knn_scratch_bytes(int64_t P);
 int h3dgs_dist_knn3(int32_t P, const float* points, float* mean_dist2, void* scratch, void* stream);
+
+/* ---- hierarchy creator (csrc/hier_build.cu; the GaussianHierarchyCreator stage of scripts/full_train.py:185-200) ----
+ * This project's own rule (upstream's creator is not available to compare with).  Input: P >= 1 Gaussians in the .hier
+ * representation: xyz [P,3], log_scales [P,3], rotations [P,4] wxyz of any norm, activated opacities [P], shs [P,16,3].
+ * Output: N = 2P - 1 nodes and N Gaussian rows, row i belongs to node i: out_xyz [N,3], out_shs [N,16,3],
+ * out_opacities [N], out_log_scales [N,3], out_rotations [N,4], out_nodes [N,7], out_boxes [N,2,4] (16-byte aligned),
+ * out_source [N] (the input index of a leaf row, -1 for a merged row).
+ *  Topology: the binary radix tree of the augmented keys (key, sorted position).  key = 63-bit Morton code, 21 bits per
+ *    axis, x in the highest bit of every triple: q = min(2097151, (uint32)((x - lo) * s)), s = 2097152.0f / (hi - lo)
+ *    (0 when hi == lo), lo / hi the bounding box of the positions, every operation rounded in fp32.  The keys are sorted
+ *    stably (input index as the value); every internal node splits its range at the highest differing bit; every leaf
+ *    holds one Gaussian.
+ *  Node order: BFS, i.e. by (level from the root, first sorted position of the range): siblings are adjacent (the lower
+ *    range first) and every level is a contiguous index range.
+ *  Nodes: {depth = height (0 at leaves), parent (-1 at the root), start = i, count_leafs = 1 | 0, count_merged = 0 | 1,
+ *    start_children (0 at a leaf), count_children = 0 | 2}.
+ *  Leaf rows: bit-exact copies of input row source[i] (the rotation stays unnormalised).
+ *  Merged rows, fp64: per leaf sigma = exp(log_scale), R from the normalised quaternion (a zero quaternion counts as the
+ *    identity), Sigma_i = R diag(sigma^2) R^T, A_i = s1 s2 + s1 s3 + s2 s3, w_i = o_i A_i.  Per node over the leaves of its
+ *    subtree: W = sum w_i, mu = sum w_i mu_i / W, Sigma = sum w_i (Sigma_i + d_i d_i^T) / W with d_i = mu_i - mu,
+ *    SH = sum w_i SH_i / W; computed from the two children carrying W, which is the same formula.  W = 0: the unweighted
+ *    mean of the two children's moments (mu, Sigma with the d d^T term, SH).  Eigenvalues of Sigma floored at 1e-24 give
+ *    log_scale = log(sqrt(lambda)), in descending order, and opacity = W / A(sqrt(lambda)) (not clamped; W = 0 gives 0);
+ *    the eigenvectors give the rotation: unit, right-handed, w >= 0.
+ *  Boxes: a leaf's is mu +- 3 sqrt(diag Sigma_i) rounded to fp32, an interior node's the fp32 union of its children's
+ *    (nesting is exact); min.w = largest extent (fp32 max - min), max.w = 0.
+ * H3DGS_EINVAL: P < 1, P > 2^30, a NULL pointer, out_boxes not 16-byte aligned, a non-finite position, log-scale or
+ * rotation component, a log-scale above 300 (its square would overflow the fp64 moments), or a negative or non-finite
+ * opacity (nothing is written to the outputs then).  An offline tool: it synchronises `stream` (twice), and returns
+ * after enqueueing the last merge.  The result depends only on the input.  scratch: >= h3dgs_build_hierarchy_scratch_bytes(P)
+ * device bytes, 256-byte aligned (0 for P out of range): about 1 kB per input Gaussian (fp64 moments and SH of the
+ * 2P - 1 nodes), so memory, not the 2^30 limit, bounds P in practice (some 70 M Gaussians on an 80 GB device). */
+size_t h3dgs_build_hierarchy_scratch_bytes(int64_t P);
+int h3dgs_build_hierarchy(int32_t P, const float* xyz, const float* log_scales, const float* rotations,
+                          const float* opacities, const float* shs, float* out_xyz, float* out_shs, float* out_opacities,
+                          float* out_log_scales, float* out_rotations, int32_t* out_nodes, float* out_boxes,
+                          int32_t* out_source, void* scratch, void* stream);
 
 /* ---- sparse Adam (SURVEY.md 8f-4; replaces scene/OurAdam.py:249-337 as driven by train_single.py:170-178) ----
  * In-place Adam update of the rows listed in relevant[num_relevant] (int64 row indices) of one parameter
