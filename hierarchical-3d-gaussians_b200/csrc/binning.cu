@@ -78,7 +78,7 @@ identify_tile_ranges_kernel(int64_t D, const uint64_t* __restrict__ keys, uint32
     if (i == D - 1) ranges[2 * tile + 1] = (uint32_t)D;
 }
 
-// kbits of the per-tile SORTED record copy: bits 0..11 num_node_kids (saturated), bits 16..31 the block mask.
+// kbits of the per-tile SORTED record copy: bits 0..15 num_node_kids (saturated at 65535), bits 16..31 the block mask.
 // (The unsorted record keeps K1's layout: kids in bits 0..19, SH clamp flags in 20..22.)
 __device__ __forceinline__ uint32_t sorted_kbits(uint32_t kbits, uint32_t mask16) {
     return min(kbits & kKidsMask, kSortedKidsMask) | (mask16 << kBlockShift);

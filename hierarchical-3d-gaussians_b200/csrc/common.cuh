@@ -22,16 +22,17 @@ constexpr float kTStop = 0.0001f;
 constexpr float kWEps = 0.0000001f;
 constexpr uint32_t kKidsMask = 0xFFFFFu;
 constexpr int kClampShift = 20;
-// per-tile sorted record copy: kids saturate at 12 bits, the upper half holds the reach mask of the tile's
-// sixteen 4x4-pixel blocks (binning.cu::block_mask16)
-constexpr uint32_t kSortedKidsMask = 0xFFFu;
+// per-tile sorted record copy: kids saturate at 16 bits (65535, the largest count the blend kernels see), the upper
+// half holds the reach mask of the tile's sixteen 4x4-pixel blocks (binning.cu::block_mask16)
+constexpr uint32_t kSortedKidsMask = 0xFFFFu;
 constexpr int kBlockShift = 16;
 
 // Per-Gaussian projected record: 3 x float4 = 48 B, 16-B aligned, so a batch of
 // records is one contiguous cp.async.bulk (TMA) transfer.
 //   a = {x, y, conic.x, conic.y}
-//   b = {conic.z, opacity, t, kbits}     kbits: bits 0..19 num_node_kids, 20..22 SH clamp flags; the per-tile
-//                                        SORTED copy instead holds kids in bits 0..11 and, in bits 16..31, the mask
+//   b = {conic.z, opacity, t, kbits}     kbits: bits 0..19 num_node_kids (k <= 1 stored as 1, saturated at 2^20 - 1),
+//                                        20..22 SH clamp flags; the per-tile
+//                                        SORTED copy instead holds kids in bits 0..15 (saturated at 65535) and, in bits 16..31, the mask
 //                                        of the tile's sixteen 4x4-pixel blocks this entry can reach (binning.cu)
 //   c = {r, g, b, invdepth}
 struct __align__(16) Record { float4 a, b, c; };

@@ -21,7 +21,7 @@ struct float4 { float x, y, z, w; };
 constexpr float kAlphaCap = 0.99f;
 constexpr float kAlphaSkip = 1.0f / 255.0f;
 constexpr float kTStop = 0.0001f;
-constexpr uint32_t kSortedKidsMask = 0xFFFu;
+constexpr uint32_t kSortedKidsMask = 0xFFFFu;
 #endif
 struct f2 { float lo, hi; };
 H3_PM_FN f2 pk(float lo, float hi) { return f2{lo, hi}; }
@@ -91,8 +91,8 @@ H3_PM_FN void pair_gauss(f2 power, float opacity, f2& G, f2& abase) {
 // per-entry, so the early out is warp-uniform.  GRAD = false drops the derivative da'/da.
 // 1 - (1-a)^(1/k) = -expm1(log1p(-a)/k).  Near the 1/255 skip threshold a is small and the direct form
 // cancels catastrophically (abs error ~2e-7 on a value ~4e-3 moves the skip decision for 100x more
-// pixels than in flat mode), so small a uses the two series (relative error < 2e-7); larger a goes
-// through MUFU.LG2 / MUFU.EX2.
+// pixels than in flat mode), so a small result uses the series of expm1 (relative error < 2e-7 from the series, plus
+// MUFU.LG2's ~2^-22 absolute error on log2(1-a) for a >= 1/16); a large one goes through MUFU.EX2.
 template <bool HIER, bool GRAD>
 H3_PM_FN void pair_hier_alpha(f2 a, float t, uint32_t k /* num_node_kids */, f2& alpha, f2& dadb) {
     alpha = a; dadb = bc(1.0f);
@@ -120,19 +120,21 @@ H3_PM_FN void pair_hier_alpha(f2 a, float t, uint32_t k /* num_node_kids */, f2&
     }
     const float ik = fast_rcp((float)k);
     const f2 l2 = pk(fast_log2(o0), fast_log2(o1));
-    // -log1p(-a) = a (1 + a/2 + a^2/3 + a^3/4 + a^4/5);  yn = -log1p(-a)/k >= 0
+    // yn = -log1p(-a)/k >= 0: for small a the series -log1p(-a) = a (1 + a/2 + a^2/3 + a^3/4 + a^4/5), else -ln2 lg2(1-a)
     f2 L = fma2(a, bc(0.2f), bc(0.25f));
     L = fma2(a, L, bc(0.33333334f));
     L = fma2(a, L, bc(0.5f));
     L = fma2(a, L, bc(1.0f));
-    const f2 yn = mul2(mul2(a, L), bc(ik));
-    // -expm1(-yn) = yn (1 - yn/2 + yn^2/6 - yn^3/24)
+    const f2 yn = sel2(a0 < 0.0625f, a1 < 0.0625f, mul2(mul2(a, L), bc(ik)), mul2(l2, bc(-0.6931472f * ik)));
+    // -expm1(-yn) = yn (1 - yn/2 + yn^2/6 - yn^3/24).  The switch is on yn, not on a: for large k a moderate a gives a
+    // small 1 - (1-a)^(1/k), where 1 - MUFU.EX2 would cancel (abs error ~2^-22 on a value near the 1/255 cut)
     f2 S = fma2(yn, bc(-0.041666668f), bc(0.16666667f));
     S = fma2(yn, S, bc(-0.5f));
     S = fma2(yn, S, bc(1.0f));
     const f2 omr_series = mul2(yn, S);
     const f2 omr_mufu = sub2(bc(1.0f), ex2_2(mul2(l2, bc(ik))));
-    const f2 omr = sel2(a0 < 0.0625f, a1 < 0.0625f, omr_series, omr_mufu);
+    float y0, y1; upk(yn, y0, y1);
+    const f2 omr = sel2(y0 < 0.0625f, y1 < 0.0625f, omr_series, omr_mufu);
     alpha = fma2(bc(u), omr, mul2(bc(t), a));
     if (GRAD) dadb = fma2(bc(u * ik), ex2_2(mul2(l2, bc(ik - 1.0f))), bc(t));
 }

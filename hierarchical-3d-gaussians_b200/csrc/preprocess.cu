@@ -170,8 +170,10 @@ preprocess_kernel(int P, const float* __restrict__ means3D, const float* __restr
                 Record rec;
                 rec.a = make_float4(ix, iy, conx, cony);
                 const float tt = ts ? ts[i] : 1.0f;
-                const uint32_t k = kids ? (uint32_t)kids[i] : 1u;
-                rec.b = make_float4(conz, LERP(opacities[c], opacities[p]), tt, __uint_as_float((k & kKidsMask) | clampbits));
+                // k <= 1 (negative included) is the identity; larger counts saturate instead of wrapping in the 20-bit field
+                const int32_t kin = kids ? kids[i] : 1;
+                const uint32_t k = kin <= 1 ? 1u : min((uint32_t)kin, kKidsMask);
+                rec.b = make_float4(conz, LERP(opacities[c], opacities[p]), tt, __uint_as_float(k | clampbits));
                 rec.c = make_float4(rgb[0], rgb[1], rgb[2], 1.0f / vz);
                 records[i] = rec;
                 depths[i] = vz;

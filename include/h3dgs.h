@@ -85,7 +85,8 @@ typedef struct h3dgs_raster_args {
     const float* cov3D_precomp; /* [P,6] xx,xy,xz,yy,yz,zz or NULL                              */
     /* hierarchy extras (empty tensors at the flat call sites -> NULL) */
     const float* interpolation_weights; /* t  [>=P] or NULL                                     */
-    const int32_t* num_node_kids;       /* k  [>=P] or NULL                                     */
+    const int32_t* num_node_kids;       /* k  [>=P] or NULL; k <= 1 (negative included) is the
+                                           identity, counts above 65535 render as 65535          */
     /* In-kernel cut gather + parent lerp (GaussianRasterizationSettings.render_indices /
      * parent_indices; empty at the shipped call sites, SURVEY.md 8a note 1).  When
      * render_indices != NULL the per-Gaussian inputs above are the FULL arrays with

@@ -52,6 +52,17 @@ def splat(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_prec
           viewmatrix, projmatrix, campos, bg, W, H, tanfovx, tanfovy, sh_degree=3, scale_modifier=1.0,
           ts=None, kids=None, do_depth=False):
     """All tensor args torch (any float dtype, CPU).  Returns (color[3,H,W], radii[P], invdepth[1,H,W])."""
+    pr = project(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix, projmatrix,
+                 campos, W, H, tanfovx, tanfovy, sh_degree, scale_modifier)
+    color, invd = blend2d(pr["px"], pr["py"], pr["conic"], pr["opacities"], pr["rgb"], pr["depth"], pr["visible"],
+                          pr["rect"], bg, W, H, ts, kids, do_depth)
+    return color, pr["radii"], invd
+
+
+def project(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+            viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, sh_degree=3, scale_modifier=1.0):
+    """The per-Gaussian half of splat: the 2D Gaussians blend2d takes (px, py, conic, opacities, rgb, depth = view z,
+    visible, rect) and radii, as a dict."""
     dt = means3D.dtype
     P = means3D.shape[0]
     V = viewmatrix.reshape(4, 4).to(dt); PM = projmatrix.reshape(4, 4).to(dt)
@@ -97,9 +108,18 @@ def splat(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_prec
         d = means3D - campos[None].to(dt)
         d = d / d.norm(dim=1, keepdim=True)
         rgb = torch.clamp_min(eval_sh(sh_degree, shs, d) + 0.5, 0.0)
+    return dict(px=px, py=py, conic=conic, opacities=opacities.reshape(-1), rgb=rgb, depth=pv[:, 2], visible=visible,
+                rect=(rminx, rmaxx, rminy, rmaxy), radii=radii)
+
+
+def blend2d(px, py, conic, opacities, rgb, depth, visible, rect, bg, W, H, ts=None, kids=None, do_depth=False):
+    """The blend over projected 2D Gaussians: px, py [P], conic [P,3], opacities [P], rgb [P,3], depth [P] (view z),
+    visible [P] bool, rect = (rminx, rmaxx, rminy, rmaxy) in tiles.  Returns (color[3,H,W], invdepth[1,H,W] or None)."""
+    dt = px.dtype
+    rminx, rmaxx, rminy, rmaxy = rect
     # depth order, ties by index (stable), visible only
     idx = torch.nonzero(visible).flatten()
-    order = idx[torch.argsort(pv[idx, 2].detach().float(), stable=True)]
+    order = idx[torch.argsort(depth[idx].detach().float(), stable=True)]
     ys, xs = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
     pixx = xs.reshape(-1, 1).to(dt); pixy = ys.reshape(-1, 1).to(dt)
     tlx = (xs.reshape(-1, 1) // TILE).to(dt); tly = (ys.reshape(-1, 1) // TILE).to(dt)
@@ -108,7 +128,7 @@ def splat(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_prec
     dx = px[o][None] - pixx; dy = py[o][None] - pixy
     power = -0.5 * (conic[o, 0][None] * dx * dx + conic[o, 2][None] * dy * dy) - conic[o, 1][None] * dx * dy
     G = torch.exp(torch.clamp(power, max=0.0))
-    araw = opacities.reshape(-1)[o][None] * G
+    araw = opacities[o][None] * G
     alpha = araw + (torch.clamp(araw, max=0.99) - araw).detach()      # cap not differentiated (published bwd)
     if ts is not None and ts.numel() > 0:
         t = ts.reshape(-1)[o][None].to(dt); k = kids.reshape(-1)[o][None].to(dt)
@@ -126,5 +146,5 @@ def splat(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_prec
     color = color.t().reshape(3, H, W)
     invd = None
     if do_depth:
-        invd = (w @ (1.0 / pv[o, 2])[:, None]).reshape(1, H, W) if o.numel() else torch.zeros(1, H, W, dtype=dt)
-    return color, radii, invd
+        invd = (w @ (1.0 / depth[o])[:, None]).reshape(1, H, W) if o.numel() else torch.zeros(1, H, W, dtype=dt)
+    return color, invd

@@ -22,7 +22,7 @@ static void ref_alpha(const Entry& e, double px, double py, bool hier, double& p
     double a = fmin(0.99, e.b.y * G);
     alpha = a; dadb = 1.0;
     union { float f; uint32_t u; } kb; kb.f = e.b.w;
-    const uint32_t k = kb.u & 0xFFFu;
+    const uint32_t k = kb.u & 0xFFFFu;              // the sorted copy's 16-bit field
     const double t = e.b.z;
     if (hier && k > 1 && t < 1.0) {
         alpha = t * a + (1 - t) * (1 - pow(1 - a, 1.0 / k));
@@ -86,7 +86,12 @@ static int run(int trial, bool verbose) {
         e.a.z = (float)(sy * sy / det); e.a.w = (float)(-rho * sx * sy / det); e.b.x = (float)(sx * sx / det);
         e.b.y = (float)(urand() < 0.15 ? 1.2 * urand() : 0.05 + 0.5 * urand());     // opacity may exceed 1 (hierarchy)
         e.b.z = (float)(urand() < 0.3 ? 1.0 : urand());
-        union { float f; uint32_t u; } kb; kb.u = (uint32_t)(1 + rand() % 4) | (0xFu << 24) | ((uint32_t)(rand() & 7) << 20);
+        union { float f; uint32_t u; } kb;
+        // k: mostly small families, also the wide counts up to the field's 65535 (1 - (1-a)^(1/k) then sits at the 1/255 cut
+        // for a >= 1/16); the reach mask in bits 16..31 must not leak into the count
+        const int kd = rand() % 8;
+        const uint32_t kk = kd < 5 ? 1 + rand() % 4 : kd == 5 ? 5 + rand() % 60 : kd == 6 ? 60 + rand() % 4000 : 4000 + rand() % 61536;
+        kb.u = kk | ((uint32_t)(rand() & 0xFFFF) << 16);
         e.b.w = kb.f;
         e.c.x = (float)urand(); e.c.y = (float)urand(); e.c.z = (float)urand(); e.c.w = (float)(0.05 + urand());
     }
