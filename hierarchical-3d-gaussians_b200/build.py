@@ -13,11 +13,11 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",
           "-ccbin", "/usr/bin/g++"]
 # files whose results feed integer artefacts, or whose arithmetic is pinned bit for bit (knn.cu, the Morton keys of
-# hier_build.cu), are compiled without FMA contraction
-NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu", "knn.cu", "hier_build.cu"}
+# hier_build.cu and hier_merge.cu, the merger's ownership rule), are compiled without FMA contraction
+NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu", "knn.cu", "hier_build.cu", "hier_merge.cu"}
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_forward.cu", "render_backward.cu",
            "preprocess_backward.cu", "hierarchy.cu", "loss.cu", "l1_loss.cu", "optim.cu", "peer.cu", "metrics.cu",
-           "knn.cu", "hier_build.cu"]
+           "knn.cu", "hier_build.cu", "hier_merge.cu"]
 
 
 def _needs_build(src, obj, deps):

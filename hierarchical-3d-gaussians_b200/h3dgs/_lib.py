@@ -25,6 +25,7 @@ EXPORTS = [
     "h3dgs_peer_flag_bytes", "h3dgs_peer_alloc", "h3dgs_peer_free", "h3dgs_peer_export", "h3dgs_peer_open", "h3dgs_peer_close",
     "h3dgs_peer_barrier", "h3dgs_peer_barrier_status", "h3dgs_eval_metrics",
     "h3dgs_knn_scratch_bytes", "h3dgs_dist_knn3", "h3dgs_build_hierarchy_scratch_bytes", "h3dgs_build_hierarchy",
+    "h3dgs_merge_hierarchies_scratch_bytes", "h3dgs_merge_hierarchies",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -126,6 +127,12 @@ def bind(l):
         l.h3dgs_build_hierarchy_scratch_bytes.argtypes = [C.c_int64]
         l.h3dgs_build_hierarchy.restype = C.c_int
         l.h3dgs_build_hierarchy.argtypes = [C.c_int32] + [C.c_void_p] * 15
+    if hasattr(l, "h3dgs_merge_hierarchies"):    # hierarchy merger (an emulation build has it when it compiles hier_merge.cu)
+        l.h3dgs_merge_hierarchies_scratch_bytes.restype = C.c_size_t
+        l.h3dgs_merge_hierarchies_scratch_bytes.argtypes = [C.c_int32, C.c_int64, C.c_int64]
+        l.h3dgs_merge_hierarchies.restype = C.c_int
+        l.h3dgs_merge_hierarchies.argtypes = [C.c_int32] + [C.c_void_p] * 10 + [ALLOC_FN, C.c_void_p, C.c_void_p,
+                                                                                 C.c_void_p, C.c_void_p]
     if hasattr(l, "h3dgs_l1_ssim_forward"):      # loss / optimizer kernels (absent from the emulation build)
         l.h3dgs_l1_ssim_forward.restype = C.c_int
         l.h3dgs_l1_ssim_forward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5

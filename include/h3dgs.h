@@ -10,6 +10,7 @@
  *   (both of the above, device-side, for a graph-captured step)  -> h3dgs_lod_cut
  *   simple_knn._C.distCUDA2                                      -> h3dgs_dist_knn3
  *   the GaussianHierarchyCreator executable                      -> h3dgs_build_hierarchy
+ *   the GaussianHierarchyMerger executable                       -> h3dgs_merge_hierarchies
  *
  * The reference binds those through two pip packages whose source is absent from
  * the reference checkout (empty submodules, .gitmodules:5-13); the interface is pinned by
@@ -340,6 +341,58 @@ int h3dgs_build_hierarchy(int32_t P, const float* xyz, const float* log_scales, 
                           const float* opacities, const float* shs, float* out_xyz, float* out_shs, float* out_opacities,
                           float* out_log_scales, float* out_rotations, int32_t* out_nodes, float* out_boxes,
                           int32_t* out_source, void* scratch, void* stream);
+
+/* ---- hierarchy merger (csrc/hier_merge.cu; the GaussianHierarchyMerger stage of scripts/full_train.py:241-264) ----
+ * This project's own rule (upstream's merger is not available to compare with).  Input: K >= 1 chunk hierarchies in
+ * the .hier representation, concatenated in argv order: rows xyz [M,3], shs [M,16,3], activated opacities [M],
+ * log_scales [M,3], rotations [M,4]; nodes [N,7] {depth, parent, start, count_leafs, count_merged, start_children,
+ * count_children} with chunk-local indices; boxes [N,2,4].  Chunk c owns nodes [node_offsets[c], node_offsets[c+1]) and
+ * rows [row_offsets[c], row_offsets[c+1]) (host int64 arrays of K + 1, from 0, not decreasing) and a cell
+ * cells[4c .. 4c+3] = (cx, cy, ex, ey) (host fp32: the x and y of its center.txt and extent.txt, full widths).
+ *  Rows that no node claims are dropped (the skybox train_post appends).  A leaf Gaussian is a row a node counts in
+ *    its count_leafs.
+ *  Ownership: a leaf Gaussian at (x, y) belongs to the chunk j minimising the key (k1, k2, j), in fp32 without FMA:
+ *    ax = |x - cx|, ox = max(ax - 0.5f * ex, 0) (y alike), k1 = ox*ox + oy*oy, k2 = max(ax / ex, ay / ey).  Chunk c
+ *    keeps only the leaf Gaussians it owns; merged rows are never tested.
+ *  Pieces: a node of chunk c is pure when every leaf Gaussian of its subtree is owned by c (vacuously so without
+ *    any).  Items of chunk c: every maximal pure subtree holding a leaf Gaussian, kept whole (rows, boxes, all its
+ *    descendants); every owned leaf Gaussian of an impure node, as a one-Gaussian item.  Impure nodes are dropped.
+ *    Item order: the subtree items by global node index, then the one-Gaussian items by global row index.
+ *  Top tree: the R items are the P leaves of h3dgs_build_hierarchy's tree: an item's moments (W, mu, Sigma, SH) are
+ *    that function's fp64 formulas over the leaf Gaussians of the item (W = 0: their unweighted mean), its position
+ *    for the Morton key is mu rounded to fp32; a subtree item keeps its input box, a one-Gaussian item gets the
+ *    creator's leaf box.  Summation order (fixed, so the result is repeatable): the item's leaf Gaussians in global row
+ *    order, lane l of 32 summing positions l, l + 32, ... in turn, the 32 partial sums then combined by an xor
+ *    butterfly (offsets 16, 8, 4, 2, 1).  A restatement that sums in another order, or evaluates exp differently, can
+ *    put mu on the other side of an fp32 rounding boundary and so change a Morton key (about 1e-9 per multi-Gaussian
+ *    item); a one-Gaussian item's mu rounds to its own position.  Top interior nodes get the creator's merged row,
+ *    depth 1 + the larger child depth and the union box.  R = 1: the single item is the root.
+ *  Output: nodes [0, 2R - 1) are the top tree in the creator's BFS order, its leaf slots the items; then the
+ *    non-root nodes of the kept subtrees, chunk by chunk, each in input order.  Rows follow node order, each node's
+ *    block in its input order; a top interior node holds one merged row (count_leafs 0, count_merged 1), a one-
+ *    Gaussian item one leaf row (depth 0, count_leafs 1, no children).  parent, start and start_children are
+ *    renumbered (start_children 0 without children; the start of a node without rows is where its block would begin,
+ *    at most the last row); count_children counts kept children; everything else in a kept node, and every kept row
+ *    and box, is a bit-exact copy.  source_chunk / source_row [RO]: the input chunk and chunk-local row of every output
+ *    row, -1 / -1 for a merged top row.  On creator-built inputs every node holds one row with start = its index.
+ *  Sizes: the outputs are allocated through `alloc(alloc_user, which, bytes)` once their sizes are known, after the
+ *    checks: which = 9 a work block (first; 256-byte aligned), then 0 xyz [RO,3], 1 shs [RO,16,3], 2 opacities [RO],
+ *    3 log_scales [RO,3], 4 rotations [RO,4], 5 nodes [NO,7] int32, 6 boxes [NO,2,4], 7 source_chunk [RO] int32,
+ *    8 source_row [RO] int32.  counts (host int64[3]) receives {NO, RO, R}.
+ * H3DGS_EINVAL, with nothing allocated or written: a NULL pointer, K < 1, bad offsets, no node or no row, more than
+ * 2^31 - 1 nodes plus rows; an inconsistent node table (an index out of range, a child whose parent disagrees, a row
+ * claimed by two nodes, a parent chain longer than N); a leaf Gaussian failing h3dgs_build_hierarchy's input checks; a
+ * cell with a non-finite center or an extent that is not finite and positive; no chunk owning anything; more than
+ * 2^31 - 1 output nodes or rows.  Every one of these is found before the first `alloc` call.  H3DGS_ENOMEM: `alloc`
+ * returned NULL.  An offline tool: it synchronises `stream`
+ * several times and returns after enqueueing the last copy.  The result depends only on the input (no fp64 atomics).
+ * scratch: >= h3dgs_merge_hierarchies_scratch_bytes(K, N, M) device bytes, 256-byte aligned (0 when out of range):
+ * about 50 bytes per node and row; the work block is about 1.4 kB per item. */
+size_t h3dgs_merge_hierarchies_scratch_bytes(int32_t K, int64_t total_nodes, int64_t total_rows);
+int h3dgs_merge_hierarchies(int32_t K, const int64_t* node_offsets, const int64_t* row_offsets, const float* cells,
+                            const float* xyz, const float* shs, const float* opacities, const float* log_scales,
+                            const float* rotations, const int32_t* nodes, const float* boxes, h3dgs_alloc_fn alloc,
+                            void* alloc_user, int64_t* counts, void* scratch, void* stream);
 
 /* ---- sparse Adam (SURVEY.md 8f-4; replaces scene/OurAdam.py:249-337 as driven by train_single.py:170-178) ----
  * In-place Adam update of the rows listed in relevant[num_relevant] (int64 row indices) of one parameter
