@@ -7,7 +7,9 @@
 // backward.  Here: ONE kernel forward (separable 11+11 taps in shared memory, 16x16 output tiles with a
 // 5-pixel halo, all five moments at once, SSIM + L1 partial sums, and the three derivative maps the
 // backward needs) and ONE kernel backward (the three maps convolved with the same window and combined
-// with img / gt per pixel).  With mu = G*x etc.:
+// with img / gt per pixel).  The 11 window weights travel as a by-value kernel argument, as in metrics.cu: no
+// __constant__ upload, so the first call needs no host synchronisation and may happen inside a CUDA graph capture.
+// With mu = G*x etc.:
 //   s = A1 A2 / (B1 B2),  A1 = 2 mu1 mu2 + C1, A2 = 2 s12 + C2, B1 = mu1^2 + mu2^2 + C1, B2 = s1 + s2 + C2
 //   d(sum s)/d img1 = G*(ds/dmu1) + 2 img1 (G*(ds/dE11)) + img2 (G*(ds/dE12))
 //   ds/dmu1 = 2 mu2 (A2 - A1)/(B1 B2) - s (2 mu1/B1 - 2 mu1/B2),  ds/dE11 = -s/B2,  ds/dE12 = 2 A1/(B1 B2)
@@ -16,7 +18,7 @@
 namespace h3dgs {
 
 constexpr int kR = 5, kTS = 16, kHalo = kTS + 2 * kR;      // 26
-__constant__ float c_win[11];
+struct LossWindow { float w[11]; };
 
 __device__ __forceinline__ float block_sum_256(float v, float* s_red) {
     v += __shfl_down_sync(0xffffffffu, v, 16); v += __shfl_down_sync(0xffffffffu, v, 8);
@@ -34,7 +36,7 @@ __device__ __forceinline__ float block_sum_256(float v, float* s_red) {
 
 __global__ void __launch_bounds__(256)
 l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                       double* __restrict__ sums, float* __restrict__ maps, size_t map_stride)
+                       double* __restrict__ sums, float* __restrict__ maps, size_t map_stride, const LossWindow win)
 {
     __shared__ float sa[kHalo][kHalo + 1], sb[kHalo][kHalo + 1];
     __shared__ float hz[5][kHalo][kTS];
@@ -57,7 +59,7 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
         float m1 = 0.f, m2 = 0.f, e11 = 0.f, e22 = 0.f, e12 = 0.f;
 #pragma unroll
         for (int k = 0; k < 11; k++) {
-            const float w = c_win[k], a = sa[r][x + k], b = sb[r][x + k];
+            const float w = win.w[k], a = sa[r][x + k], b = sb[r][x + k];
             m1 += w * a; m2 += w * b; e11 += w * a * a; e22 += w * b * b; e12 += w * a * b;
         }
         hz[0][r][x] = m1; hz[1][r][x] = m2; hz[2][r][x] = e11; hz[3][r][x] = e22; hz[4][r][x] = e12;
@@ -66,7 +68,7 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
     float mu1 = 0.f, mu2 = 0.f, e11 = 0.f, e22 = 0.f, e12 = 0.f;
 #pragma unroll
     for (int k = 0; k < 11; k++) {
-        const float w = c_win[k];
+        const float w = win.w[k];
         mu1 += w * hz[0][ty + k][tx]; mu2 += w * hz[1][ty + k][tx];
         e11 += w * hz[2][ty + k][tx]; e22 += w * hz[3][ty + k][tx]; e12 += w * hz[4][ty + k][tx];
     }
@@ -96,7 +98,7 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
 __global__ void __launch_bounds__(256)
 l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
                         const float* __restrict__ maps, size_t map_stride, const float* __restrict__ coeffs,
-                        float* __restrict__ dL_dimg)
+                        float* __restrict__ dL_dimg, const LossWindow win)
 {
     __shared__ float sm[3][kHalo][kHalo + 1];
     __shared__ float hz[3][kHalo][kTS];
@@ -118,7 +120,7 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
         float a0 = 0.f, a1 = 0.f, a2 = 0.f;
 #pragma unroll
         for (int k = 0; k < 11; k++) {
-            const float w = c_win[k];
+            const float w = win.w[k];
             a0 += w * sm[0][r][x + k]; a1 += w * sm[1][r][x + k]; a2 += w * sm[2][r][x + k];
         }
         hz[0][r][x] = a0; hz[1][r][x] = a1; hz[2][r][x] = a2;
@@ -127,7 +129,7 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
     float c0 = 0.f, c1 = 0.f, c2 = 0.f;
 #pragma unroll
     for (int k = 0; k < 11; k++) {
-        const float w = c_win[k];
+        const float w = win.w[k];
         c0 += w * hz[0][ty + k][tx]; c1 += w * hz[1][ty + k][tx]; c2 += w * hz[2][ty + k][tx];
     }
     const int px = bx + tx, py = by + ty;
@@ -139,19 +141,12 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
     }
 }
 
-static int upload_window(cudaStream_t s) {
-    // utils/loss_utils.py:23-25: exp(-(x - 5)^2 / (2 * 1.5^2)), normalised (fp32 tensor)
-    static bool done[64] = {false};
-    int dev = 0;
-    H3_CUDA(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && done[dev]) return H3DGS_OK;
-    float w[11]; float sum = 0.f;
-    for (int x = 0; x < 11; x++) { w[x] = (float)exp(-(double)((x - 5) * (x - 5)) / (2.0 * 1.5 * 1.5)); sum += w[x]; }
-    for (int x = 0; x < 11; x++) w[x] /= sum;
-    H3_CUDA(cudaMemcpyToSymbolAsync(c_win, w, sizeof(w), 0, cudaMemcpyHostToDevice, s));
-    H3_CUDA(cudaStreamSynchronize(s));            // w lives on the stack
-    if (dev >= 0 && dev < 64) done[dev] = true;
-    return H3DGS_OK;
+static LossWindow make_loss_window() {
+    // utils/loss_utils.py:23-25: exp(-(x - 5)^2 / (2 * 1.5^2)), normalised in fp32 (the weights of metrics.cu)
+    LossWindow w; float sum = 0.f;
+    for (int x = 0; x < 11; x++) { w.w[x] = (float)exp(-(double)((x - 5) * (x - 5)) / (2.0 * 1.5 * 1.5)); sum += w.w[x]; }
+    for (int x = 0; x < 11; x++) w.w[x] /= sum;
+    return w;
 }
 
 }  // namespace h3dgs
@@ -163,11 +158,9 @@ extern "C" int h3dgs_l1_ssim_forward(int32_t C, int32_t H, int32_t W, const floa
 {
     if (C <= 0 || H <= 0 || W <= 0 || !img || !gt || !sums) { set_error("l1_ssim_forward: bad arguments"); return H3DGS_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
-    int rc = upload_window(s);
-    if (rc) return rc;
     H3_CUDA(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
     const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, C);
-    l1_ssim_forward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)C * H * W);
+    l1_ssim_forward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)C * H * W, make_loss_window());
     H3_LAUNCHED("l1_ssim_forward", 0, s);
     return H3DGS_OK;
 }
@@ -177,10 +170,8 @@ extern "C" int h3dgs_l1_ssim_backward(int32_t C, int32_t H, int32_t W, const flo
 {
     if (C <= 0 || H <= 0 || W <= 0 || !img || !gt || !maps || !coeffs || !dL_dimg) { set_error("l1_ssim_backward: bad arguments"); return H3DGS_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
-    int rc = upload_window(s);
-    if (rc) return rc;
     const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, C);
-    l1_ssim_backward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, maps, (size_t)C * H * W, coeffs, dL_dimg);
+    l1_ssim_backward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, maps, (size_t)C * H * W, coeffs, dL_dimg, make_loss_window());
     H3_LAUNCHED("l1_ssim_backward", 0, s);
     return H3DGS_OK;
 }

@@ -133,11 +133,12 @@ def bind(l):
         l.h3dgs_merge_hierarchies.restype = C.c_int
         l.h3dgs_merge_hierarchies.argtypes = [C.c_int32] + [C.c_void_p] * 10 + [ALLOC_FN, C.c_void_p, C.c_void_p,
                                                                                  C.c_void_p, C.c_void_p]
-    if hasattr(l, "h3dgs_l1_ssim_forward"):      # loss / optimizer kernels (absent from the emulation build)
+    if hasattr(l, "h3dgs_l1_ssim_forward"):      # fused L1 + SSIM loss (an emulation build has it when it compiles loss.cu)
         l.h3dgs_l1_ssim_forward.restype = C.c_int
         l.h3dgs_l1_ssim_forward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5
         l.h3dgs_l1_ssim_backward.restype = C.c_int
         l.h3dgs_l1_ssim_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 6
+    if hasattr(l, "h3dgs_sparse_adam"):          # sparse Adam (absent from the emulation build)
         l.h3dgs_sparse_adam.restype = C.c_int
         l.h3dgs_sparse_adam.argtypes = [C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_double, C.c_double, C.c_double, C.c_double, C.c_int64, C.c_void_p]

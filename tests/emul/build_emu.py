@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "hierarchical-3d-gaussians_b200", "csrc")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_forward.cu", "render_backward.cu", "preprocess_backward.cu",
-           "hierarchy.cu", "l1_loss.cu"]
+           "hierarchy.cu", "l1_loss.cu", "loss.cu"]
 
 _LAUNCH = re.compile(r"((?:\b[\w:]+)(?:<[^<>;()]*>)?)\s*<<<(.*?)>>>\s*\(", re.S)
 

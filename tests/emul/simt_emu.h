@@ -123,6 +123,11 @@ template <class T> static inline T __shfl_up_sync(unsigned, T v, unsigned delta)
     raw = simt::warp_exchange(raw, src);                             // src < 0: own value
     T out; memcpy(&out, &raw, sizeof(T)); return out;
 }
+template <class T> static inline T __shfl_down_sync(unsigned, T v, unsigned delta) {
+    uint64_t raw = 0; memcpy(&raw, &v, sizeof(T));
+    raw = simt::warp_exchange(raw, simt::g_cur->lane + (int)delta);  // src > 31: own value
+    T out; memcpy(&out, &raw, sizeof(T)); return out;
+}
 
 // atomics: one OS thread, fibers only switch at collectives
 static inline float atomicAdd(float* p, float v) { float o = *p; *p = o + v; return o; }

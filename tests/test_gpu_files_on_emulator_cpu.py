@@ -1,7 +1,8 @@
 """CPU: the GPU test files themselves -- the same parity tests the H100 runs, with their own criteria -- executed
 against the emulation build of the kernels (H3DGS_EMULATE=1, tests/conftest.py, tests/emul/): the product's Python
 layer runs unchanged on CPU tensors and the kernels run under the SIMT emulator.  The 1080p / 4K frames are left to
-the GPU (they pass here too, in minutes); NCCL and the loss / optimizer kernels are out of the emulator's reach."""
+the GPU (they pass here too, in minutes); NCCL and the optimizer kernel are out of the emulator's reach.  The fused
+L1 + SSIM loss kernels (csrc/loss.cu) run on the emulation build in tests/test_ssim_ref_cpu.py."""
 import os
 import re
 import subprocess
