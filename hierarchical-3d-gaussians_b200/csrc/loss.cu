@@ -34,9 +34,22 @@ __device__ __forceinline__ float block_sum_256(float v, float* s_red) {
     return t;      // valid in thread 0
 }
 
+// train_post's image before the loss (render_post, gaussian_renderer/__init__.py:279-285): the exposure applied from the
+// right, y_c = sum_k img_k E[k][c] + E[c][3].  The fp32 order is pinned, ((img0 E[0][c] + img1 E[1][c]) + img2 E[2][c])
+// + E[c][3] with every product and sum rounded (no FMA contraction): the forward's clamp decision and the backward's are
+// taken on the same y, and a restatement outside the kernel reproduces it bit for bit.
+__device__ __forceinline__ float exposed(const float* __restrict__ img, size_t plane, size_t p, const float* __restrict__ E, int c) {
+    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(img[p], E[c]), __fmul_rn(img[plane + p], E[4 + c])),
+                               __fmul_rn(img[2 * plane + p], E[8 + c])), E[4 * c + 3]);
+}
+
+// kPost = false: the loss of img against gt (h3dgs_l1_ssim_forward).  kPost = true: the loss of a = clamp(y, 0, 1) * mask
+// against gt as it is, y = exposed(img) or img[c] (h3dgs_post_loss_forward; C = 3); exposure and mask may be NULL.
+template <bool kPost>
 __global__ void __launch_bounds__(256)
 l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                       double* __restrict__ sums, float* __restrict__ maps, size_t map_stride, const LossWindow win)
+                       double* __restrict__ sums, float* __restrict__ maps, size_t map_stride, const LossWindow win,
+                       const float* __restrict__ exposure, const float* __restrict__ mask)
 {
     __shared__ float sa[kHalo][kHalo + 1], sb[kHalo][kHalo + 1];
     __shared__ float hz[5][kHalo][kTS];
@@ -50,8 +63,21 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
         const int ly = i / kHalo, lx = i - ly * kHalo;
         const int gy = by + ly - kR, gx = bx + lx - kR;
         const bool in = gy >= 0 && gy < H && gx >= 0 && gx < W;
-        sa[ly][lx] = in ? ia[(size_t)gy * W + gx] : 0.f;        // zero padding (conv2d padding=5)
-        sb[ly][lx] = in ? ib[(size_t)gy * W + gx] : 0.f;
+        if (kPost) {
+            float a = 0.f, b = 0.f;                             // zero padding (conv2d padding=5)
+            if (in) {
+                const size_t p = (size_t)gy * W + gx;
+                const float y = exposure ? exposed(img, plane, p, exposure, c) : ia[p];
+                a = fminf(fmaxf(y, 0.f), 1.f);
+                if (mask) a *= mask[p];
+                b = ib[p];                                      // the loader clamped and masked the target already
+            }
+            sa[ly][lx] = a;
+            sb[ly][lx] = b;
+        } else {
+            sa[ly][lx] = in ? ia[(size_t)gy * W + gx] : 0.f;    // zero padding (conv2d padding=5)
+            sb[ly][lx] = in ? ib[(size_t)gy * W + gx] : 0.f;
+        }
     }
     __syncthreads();
     for (int i = tid; i < kHalo * kTS; i += 256) {
@@ -95,15 +121,13 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
     if (tid == 0) { atomicAdd(sums, (double)l1_sum); atomicAdd(sums + 1, (double)ss_sum); }
 }
 
-__global__ void __launch_bounds__(256)
-l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                        const float* __restrict__ maps, size_t map_stride, const float* __restrict__ coeffs,
-                        float* __restrict__ dL_dimg, const LossWindow win)
+// The three derivative maps of channel c convolved with the window at this thread's pixel: a horizontal and a vertical
+// 11-tap pass through shared memory over the 26x26 halo of the tile at (bx, by), zero outside the frame.
+__device__ __forceinline__ void conv_maps(int H, int W, int bx, int by, int c, const float* __restrict__ maps,
+                                          size_t map_stride, const LossWindow& win, float (&sm)[3][kHalo][kHalo + 1],
+                                          float (&hz)[3][kHalo][kTS], float& c0, float& c1, float& c2)
 {
-    __shared__ float sm[3][kHalo][kHalo + 1];
-    __shared__ float hz[3][kHalo][kTS];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int bx = blockIdx.x * kTS, by = blockIdx.y * kTS, c = blockIdx.z;
     const size_t plane = (size_t)H * W;
     for (int i = tid; i < kHalo * kHalo; i += 256) {
         const int ly = i / kHalo, lx = i - ly * kHalo;
@@ -126,12 +150,26 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
         hz[0][r][x] = a0; hz[1][r][x] = a1; hz[2][r][x] = a2;
     }
     __syncthreads();
-    float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+    c0 = 0.f; c1 = 0.f; c2 = 0.f;
 #pragma unroll
     for (int k = 0; k < 11; k++) {
         const float w = win.w[k];
         c0 += w * hz[0][ty + k][tx]; c1 += w * hz[1][ty + k][tx]; c2 += w * hz[2][ty + k][tx];
     }
+}
+
+__global__ void __launch_bounds__(256)
+l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                        const float* __restrict__ maps, size_t map_stride, const float* __restrict__ coeffs,
+                        float* __restrict__ dL_dimg, const LossWindow win)
+{
+    __shared__ float sm[3][kHalo][kHalo + 1];
+    __shared__ float hz[3][kHalo][kTS];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int bx = blockIdx.x * kTS, by = blockIdx.y * kTS, c = blockIdx.z;
+    const size_t plane = (size_t)H * W;
+    float c0, c1, c2;
+    conv_maps(H, W, bx, by, c, maps, map_stride, win, sm, hz, c0, c1, c2);
     const int px = bx + tx, py = by + ty;
     if (px < W && py < H) {
         const size_t o = (size_t)c * plane + (size_t)py * W + px;
@@ -139,6 +177,74 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
         const float sgn = (a > b) ? 1.f : ((a < b) ? -1.f : 0.f);
         dL_dimg[o] = coeffs[0] * sgn + coeffs[1] * (c0 + 2.f * a * c1 + b * c2);
     }
+}
+
+// Backward of the post loss: one CTA per 16x16 tile, looping over the three channels, because the exposure's transpose
+// needs all three dL/dy_c of a pixel.  Per channel, with a = clamp(y_c, 0, 1) * m recomputed as the forward stages it:
+//   dL/dy_c = [0 <= y_c <= 1] * (m * (k0 sign(a - b) + k1 (c0 + 2 a c1 + b c2)))      (torch's clamp passes both ends)
+// kept in registers; then dL/dimg_k = (E[k][0] g_0 + E[k][1] g_1) + E[k][2] g_2 (rounded in that order), or g_k
+// without an exposure.  dL/dimg is written once; no dL/da buffer.
+__global__ void __launch_bounds__(256)
+post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                          const float* __restrict__ exposure, const float* __restrict__ mask,
+                          const float* __restrict__ maps, size_t map_stride, const float* __restrict__ coeffs,
+                          float* __restrict__ dL_dimg, const LossWindow win)
+{
+    __shared__ float sm[3][kHalo][kHalo + 1];
+    __shared__ float hz[3][kHalo][kTS];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int bx = blockIdx.x * kTS, by = blockIdx.y * kTS;
+    const size_t plane = (size_t)H * W;
+    const int px = bx + tx, py = by + ty;
+    const bool own = px < W && py < H;
+    const size_t p = own ? (size_t)py * W + px : 0;
+    const float k0 = coeffs[0], k1 = coeffs[1];
+    const float m = (own && mask) ? mask[p] : 1.f;
+    float g[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        if (c) __syncthreads();                             // the previous channel's passes are done with sm and hz
+        float c0, c1, c2;
+        conv_maps(H, W, bx, by, c, maps, map_stride, win, sm, hz, c0, c1, c2);
+        g[c] = 0.f;
+        if (own) {
+            const float y = exposure ? exposed(img, plane, p, exposure, c) : img[(size_t)c * plane + p];
+            float a = fminf(fmaxf(y, 0.f), 1.f);
+            if (mask) a *= m;
+            const float b = gt[(size_t)c * plane + p];
+            const float sgn = (a > b) ? 1.f : ((a < b) ? -1.f : 0.f);
+            float d = k0 * sgn + k1 * (c0 + 2.f * a * c1 + b * c2);
+            if (mask) d = __fmul_rn(m, d);
+            g[c] = (y >= 0.f && y <= 1.f) ? d : 0.f;
+        }
+    }
+    if (!own) return;
+    if (exposure) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const float* Ek = exposure + 4 * k;
+            dL_dimg[(size_t)k * plane + p] =
+                __fadd_rn(__fadd_rn(__fmul_rn(Ek[0], g[0]), __fmul_rn(Ek[1], g[1])), __fmul_rn(Ek[2], g[2]));
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < 3; k++) dL_dimg[(size_t)k * plane + p] = g[k];
+    }
+}
+
+// One thread: the eight status words of the post-loss step (h3dgs/poststep.py) -- loss, L1, SSIM, rows the cut needs, D,
+// longest tile list, binning overflow, row overflow.
+__global__ void post_step_status_kernel(const double* __restrict__ sums, double inv_numel, double lambda_dssim,
+                                        const int* __restrict__ count, int extra_rows, int row_capacity,
+                                        const uint32_t* __restrict__ scan_info, double* __restrict__ out)
+{
+    const double l1 = sums[0] * inv_numel, ssim = sums[1] * inv_numel;
+    const double rows = (double)(*count + extra_rows);
+    out[0] = (1.0 - lambda_dssim) * l1 + lambda_dssim * (1.0 - ssim);
+    out[1] = l1; out[2] = ssim;
+    out[3] = rows;
+    out[4] = (double)scan_info[0]; out[5] = (double)scan_info[1]; out[6] = (double)scan_info[2];
+    out[7] = rows > (double)row_capacity ? 1.0 : 0.0;
 }
 
 static LossWindow make_loss_window() {
@@ -160,7 +266,7 @@ extern "C" int h3dgs_l1_ssim_forward(int32_t C, int32_t H, int32_t W, const floa
     cudaStream_t s = (cudaStream_t)stream;
     H3_CUDA(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
     const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, C);
-    l1_ssim_forward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)C * H * W, make_loss_window());
+    l1_ssim_forward_kernel<false><<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)C * H * W, make_loss_window(), nullptr, nullptr);
     H3_LAUNCHED("l1_ssim_forward", 0, s);
     return H3DGS_OK;
 }
@@ -173,5 +279,38 @@ extern "C" int h3dgs_l1_ssim_backward(int32_t C, int32_t H, int32_t W, const flo
     const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, C);
     l1_ssim_backward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, maps, (size_t)C * H * W, coeffs, dL_dimg, make_loss_window());
     H3_LAUNCHED("l1_ssim_backward", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_post_loss_forward(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure,
+                                       const float* mask, double* sums, float* maps, void* stream)
+{
+    if (H <= 0 || W <= 0 || !img || !gt || !sums) { set_error("post_loss_forward: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    H3_CUDA(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
+    const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 3);
+    l1_ssim_forward_kernel<true><<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)3 * H * W, make_loss_window(), exposure, mask);
+    H3_LAUNCHED("post_loss_forward", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_post_loss_backward(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure,
+                                        const float* mask, const float* maps, const float* coeffs, float* dL_dimg, void* stream)
+{
+    if (H <= 0 || W <= 0 || !img || !gt || !maps || !coeffs || !dL_dimg) { set_error("post_loss_backward: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 1);
+    post_loss_backward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, exposure, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, make_loss_window());
+    H3_LAUNCHED("post_loss_backward", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_post_step_status(const double* sums, double inv_numel, double lambda_dssim, const int32_t* count,
+                                      int32_t extra_rows, int32_t row_capacity, const uint32_t* scan_info, double* out, void* stream)
+{
+    if (!sums || !count || !scan_info || !out) { set_error("post_step_status: NULL argument"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    post_step_status_kernel<<<1, 1, 0, s>>>(sums, inv_numel, lambda_dssim, count, extra_rows, row_capacity, scan_info, out);
+    H3_LAUNCHED("post_step_status", 0, s);
     return H3DGS_OK;
 }

@@ -26,6 +26,7 @@ EXPORTS = [
     "h3dgs_peer_barrier", "h3dgs_peer_barrier_status", "h3dgs_eval_metrics",
     "h3dgs_knn_scratch_bytes", "h3dgs_dist_knn3", "h3dgs_build_hierarchy_scratch_bytes", "h3dgs_build_hierarchy",
     "h3dgs_merge_hierarchies_scratch_bytes", "h3dgs_merge_hierarchies",
+    "h3dgs_post_loss_forward", "h3dgs_post_loss_backward", "h3dgs_post_step_status",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -138,6 +139,13 @@ def bind(l):
         l.h3dgs_l1_ssim_forward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5
         l.h3dgs_l1_ssim_backward.restype = C.c_int
         l.h3dgs_l1_ssim_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 6
+        l.h3dgs_post_loss_forward.restype = C.c_int
+        l.h3dgs_post_loss_forward.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
+        l.h3dgs_post_loss_backward.restype = C.c_int
+        l.h3dgs_post_loss_backward.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 8
+        l.h3dgs_post_step_status.restype = C.c_int
+        l.h3dgs_post_step_status.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int32, C.c_int32,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]
     if hasattr(l, "h3dgs_sparse_adam"):          # sparse Adam (absent from the emulation build)
         l.h3dgs_sparse_adam.restype = C.c_int
         l.h3dgs_sparse_adam.argtypes = [C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -184,6 +184,19 @@ def l1_step(scene, cam, bg, gt, threshold=None, sh_degree=3, fused=True, gt_read
     return loss, radii, n
 
 
+def post_step(scene, cam, bg, gt, threshold, lambda_dssim=0.2, exposure=None, mask=None, sh_degree=3):
+    """One step of train_post's loop body (train_post.py:91-142) on the exact path: render_hier_fused, then the objective
+    (exposure, clamp, alpha mask, (1-l) L1 + l (1 - SSIM): h3dgs.loss.post_loss), then backward.  Gradients land in the
+    scene's tensors.  Also the path that re-runs a frame h3dgs.poststep.GraphedPostStep flagged as overflowed.
+    -> ((loss, l1, ssim) device scalars, radii, n cut rows)"""
+    from .loss import post_loss
+    scene.zero_grad()
+    img, radii, n = render_hier_fused(scene, cam, bg, threshold, sh_degree)
+    loss, l1, ssim = post_loss(img, gt, lambda_dssim, exposure, mask)
+    loss.backward()
+    return (loss, l1, ssim), radii, n
+
+
 def fov_threshold(tau, cam):
     """render_hierarchy.py:55-56"""
     return (2 * (tau + 0.5)) * cam.tanfovx / (0.5 * cam.W)

@@ -255,6 +255,31 @@ int h3dgs_l1_ssim_forward(int32_t C, int32_t H, int32_t W, const float* img, con
 int h3dgs_l1_ssim_backward(int32_t C, int32_t H, int32_t W, const float* img, const float* gt, const float* maps,
                            const float* coeffs, float* dL_dimg, void* stream);
 
+/* ---- train_post's objective (train_post.py:134-142 on render_post's exposure and clamp, gaussian_renderer/__init__.py:279-285),
+ * fused into the loss kernels above.  img [3,H,W] is the raw rasterizer output, gt [3,H,W] the target as the loader leaves
+ * it (already clamped and masked: it is neither clamped nor masked here), exposure a DEVICE [3][4] matrix or NULL (=
+ * identity), mask a DEVICE [H,W] alpha mask or NULL (= ones).  Per pixel and channel c:
+ *   y_c = exposure ? ((img_0 E[0][c] + img_1 E[1][c]) + img_2 E[2][c]) + E[c][3] : img_c    (every product and sum rounded
+ *         in this order: image.permute(1,2,0) @ E[:3,:3] + E[:3,3])
+ *   a_c = clamp(y_c, 0, 1) * mask
+ * forward: sums[0] = sum |a - gt|, sums[1] = sum of the SSIM map of (a, gt) (device doubles, zeroed here); maps [3][3,H,W]
+ *          (ds/dmu1, ds/dE11, ds/dE12 at a) are written when non-NULL (needed by backward).
+ * backward: dL/dy_c = [0 <= y_c <= 1] * mask * (coeffs[0] sign(a_c - gt_c) + coeffs[1] d(sum ssim)/d a_c),
+ *          dL_dimg_k = (E[k][0] dL/dy_0 + E[k][1] dL/dy_1) + E[k][2] dL/dy_2 (or dL/dy_k without exposure); coeffs is a
+ *          DEVICE pointer to two floats.  There is no gradient to the exposure or the mask.
+ * With exposure and mask NULL and img in [0, 1] both equal h3dgs_l1_ssim_forward / _backward with C = 3, bit for bit.
+ * Nothing synchronises with the host: exposure and mask may change between replays of a CUDA graph. */
+int h3dgs_post_loss_forward(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure, const float* mask,
+                            double* sums, float* maps, void* stream);
+int h3dgs_post_loss_backward(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure, const float* mask,
+                             const float* maps, const float* coeffs, float* dL_dimg, void* stream);
+/* Status words of the sync-free post-loss step, written by one device thread: out[0] = loss = (1 - lambda) L1 + lambda
+ * (1 - SSIM), out[1] = L1 = sums[0] * inv_numel, out[2] = SSIM = sums[1] * inv_numel, out[3] = *count + extra_rows (rows
+ * the cut needs), out[4..6] = scan_info[0..2] (D, longest tile list, binning overflow), out[7] = 1 when out[3] >
+ * row_capacity. */
+int h3dgs_post_step_status(const double* sums, double inv_numel, double lambda_dssim, const int32_t* count, int32_t extra_rows,
+                           int32_t row_capacity, const uint32_t* scan_info, double* out, void* stream);
+
 /* L1 loss and its gradient in one pass (the loss of bench.py's step; train_post.py:134-142 with lambda_dssim = 0):
  * *loss_sum [device double, zeroed here] = sum |img - gt|, dL_dimg = sign(img - gt) * scale (scale = 1 / numel for the
  * mean).  With shard_count > 1 only the 16-pixel tile rows y_tile % shard_count == shard_index are visited (loss_sum is
