@@ -1,5 +1,7 @@
 // l1_loss.cu -- L1 loss and its gradient in one pass (the loss of the step bench.py and h3dgs.graphstep time:
 // train_post.py:134-142 with lambda_dssim = 0; the SSIM term lives in loss.cu).
+// Also the two per-step kernels of train_single.py beside its photometric loss: the inverse-depth L1 with its gradient
+// (:111-117) and the densification statistics (:147-148).
 #include <algorithm>
 #include "common.cuh"
 
@@ -80,9 +82,94 @@ __global__ void step_status_kernel(double* __restrict__ loss_sum, double inv_num
     if (reset_loss) *loss_sum = 0.0;
 }
 
+// train_single's inverse-depth term (train_single.py:111-117) and its gradient in ONE pass:
+//   t = (invdepth - mono) * depth_mask (difference and product rounded), *sum += |t| (unweighted: Ll1depth_pure before
+//   the mean), dL/dinvdepth = ((w / (H W)) * sign(t)) * depth_mask with sign(0) = 0 as torch.abs; w is read on the device.
+__device__ __forceinline__ float invdepth_term(float d, float m, float k, float scale, float& acc) {
+    const float t = __fmul_rn(__fadd_rn(d, -m), k);
+    acc += fabsf(t);
+    return __fmul_rn(t > 0.f ? scale : (t < 0.f ? -scale : 0.f), k);
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256)
+invdepth_l1_grad_kernel(size_t total, float pixels, const float* __restrict__ invdepth, const float* __restrict__ mono,
+                        const float* __restrict__ depth_mask, const float* __restrict__ weight,
+                        float* __restrict__ dL_dinvdepth, double* __restrict__ sum)
+{
+    __shared__ float s_red[8];
+    const float scale = *weight / pixels;                   // IEEE division, rounded once
+    float acc = 0.f;
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total / VEC; i += (size_t)gridDim.x * 256) {
+        if (VEC == 1) { dL_dinvdepth[i] = invdepth_term(invdepth[i], mono[i], depth_mask[i], scale, acc); continue; }
+        const float4 d = reinterpret_cast<const float4*>(invdepth)[i], m = reinterpret_cast<const float4*>(mono)[i];
+        const float4 k = reinterpret_cast<const float4*>(depth_mask)[i];
+        float4 g;
+        g.x = invdepth_term(d.x, m.x, k.x, scale, acc); g.y = invdepth_term(d.y, m.y, k.y, scale, acc);
+        g.z = invdepth_term(d.z, m.z, k.z, scale, acc); g.w = invdepth_term(d.w, m.w, k.w, scale, acc);
+        reinterpret_cast<float4*>(dL_dinvdepth)[i] = g;
+    }
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const float t = warp_sum(threadIdx.x < 8 ? s_red[threadIdx.x] : 0.f);
+        if (threadIdx.x == 0 && t != 0.f) atomicAdd(sum, (double)t);
+    }
+}
+
+// The densification statistics of one training step (train_single.py:147, scene/gaussian_model.py:687-689), one thread
+// per row; rows with radii <= 0 are untouched.  The norm is sqrt(x*x + y*y) with both products, the sum and the root
+// rounded to fp32 (no FMA); the maxima propagate a NaN as torch.max does.  An overflowed capacity-mode frame
+// (scan_info[2] != 0) changes nothing: its radii are those of the real frame (the preprocess runs before the overflow
+// is known) but its gradients are zero, and the caller re-runs it.
+__global__ void __launch_bounds__(256)
+densify_stats_kernel(int P, const int* __restrict__ radii, const float* __restrict__ dL_dmeans2D, float* __restrict__ max_radii2D,
+                     float* __restrict__ xyz_gradient_accum, float* __restrict__ denom, const uint32_t* __restrict__ scan_info)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= P || (scan_info && scan_info[2])) return;
+    const int r = radii[i];
+    if (r <= 0) return;
+    const float rf = (float)r, mr = max_radii2D[i];
+    max_radii2D[i] = (mr != mr || mr > rf) ? mr : rf;
+    const float x = dL_dmeans2D[3 * (size_t)i], y = dL_dmeans2D[3 * (size_t)i + 1];
+    const float n = sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))), a = xyz_gradient_accum[i];
+    xyz_gradient_accum[i] = (n != n || n > a) ? n : a;
+    denom[i] += 1.f;
+}
+
 }  // namespace h3dgs
 
 using namespace h3dgs;
+
+extern "C" int h3dgs_invdepth_l1_grad(int32_t H, int32_t W, const float* invdepth, const float* mono, const float* depth_mask,
+                                      const float* weight, float* dL_dinvdepth, double* sum, void* stream)
+{
+    if (H <= 0 || W <= 0 || !invdepth || !mono || !depth_mask || !weight || !dL_dinvdepth || !sum) { set_error("invdepth_l1_grad: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    H3_CUDA(cudaMemsetAsync(sum, 0, sizeof(double), s));
+    const size_t total = (size_t)H * W;
+    const bool vec = (total & 3) == 0 && (((uintptr_t)invdepth | (uintptr_t)mono | (uintptr_t)depth_mask | (uintptr_t)dL_dinvdepth) & 15) == 0;
+    const int blocks = (int)std::min<size_t>(((vec ? total >> 2 : total) + 255) / 256, 132 * 16);
+    ProfScope prof(H3DGS_STAGE_INVDEPTH_L1, s);
+    if (vec) invdepth_l1_grad_kernel<4><<<blocks, 256, 0, s>>>(total, (float)total, invdepth, mono, depth_mask, weight, dL_dinvdepth, sum);
+    else invdepth_l1_grad_kernel<1><<<blocks, 256, 0, s>>>(total, (float)total, invdepth, mono, depth_mask, weight, dL_dinvdepth, sum);
+    H3_LAUNCHED("invdepth_l1_grad", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_densify_stats(int32_t P, const int32_t* radii, const float* dL_dmeans2D, float* max_radii2D,
+                                   float* xyz_gradient_accum, float* denom, const uint32_t* scan_info, void* stream)
+{
+    if (P < 0 || (P > 0 && (!radii || !dL_dmeans2D || !max_radii2D || !xyz_gradient_accum || !denom))) { set_error("densify_stats: bad arguments"); return H3DGS_EINVAL; }
+    if (P == 0) return H3DGS_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope prof(H3DGS_STAGE_DENSIFY_STATS, s);
+    densify_stats_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, radii, dL_dmeans2D, max_radii2D, xyz_gradient_accum, denom, scan_info);
+    H3_LAUNCHED("densify_stats", 0, s);
+    return H3DGS_OK;
+}
 
 extern "C" int h3dgs_step_status(double* loss_sum, double inv_numel, const int32_t* count, int32_t extra_rows, int32_t row_capacity,
                                  const uint32_t* scan_info, int32_t reset_loss, double* out, void* stream)

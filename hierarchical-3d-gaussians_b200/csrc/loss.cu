@@ -184,14 +184,20 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
 //   dL/dy_c = [0 <= y_c <= 1] * (m * (k0 sign(a - b) + k1 (c0 + 2 a c1 + b c2)))      (torch's clamp passes both ends)
 // kept in registers; then dL/dimg_k = (E[k][0] g_0 + E[k][1] g_1) + E[k][2] g_2 (rounded in that order), or g_k
 // without an exposure.  dL/dimg is written once; no dL/da buffer.
+// kGradE (train_single.py, where the exposure is a trained parameter): the same pass also leaves dL/dE [3][4] -- the
+// twelve per-pixel terms img_k * g_c (k, c < 3; one rounded product each) and g_c are summed over the CTA in fp32 (xor
+// butterfly over the warp, offsets 16 .. 1), the eight warp sums are added in fp64 in warp order and one fp64 atomic
+// per CTA and entry adds them to dL_dE.  dL/dimg does not depend on the flag.
+template <bool kGradE>
 __global__ void __launch_bounds__(256)
 post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
                           const float* __restrict__ exposure, const float* __restrict__ mask,
                           const float* __restrict__ maps, size_t map_stride, const float* __restrict__ coeffs,
-                          float* __restrict__ dL_dimg, const LossWindow win)
+                          float* __restrict__ dL_dimg, double* __restrict__ dL_dE, const LossWindow win)
 {
     __shared__ float sm[3][kHalo][kHalo + 1];
     __shared__ float hz[3][kHalo][kTS];
+    __shared__ float s_e[kGradE ? 8 : 1][12];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int bx = blockIdx.x * kTS, by = blockIdx.y * kTS;
     const size_t plane = (size_t)H * W;
@@ -218,6 +224,31 @@ post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const flo
             g[c] = (y >= 0.f && y <= 1.f) ? d : 0.f;
         }
     }
+    if (kGradE) {
+        float v[12];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const float ik = own ? img[(size_t)k * plane + p] : 0.f;
+#pragma unroll
+            for (int c = 0; c < 3; c++) v[4 * k + c] = __fmul_rn(ik, g[c]);         // dL/dE[k][c]
+            v[4 * k + 3] = g[k];                                                     // dL/dE[k][3]
+        }
+#pragma unroll
+        for (int j = 0; j < 12; j++) {
+            float t = v[j];
+            t += __shfl_xor_sync(0xffffffffu, t, 16); t += __shfl_xor_sync(0xffffffffu, t, 8);
+            t += __shfl_xor_sync(0xffffffffu, t, 4);  t += __shfl_xor_sync(0xffffffffu, t, 2);
+            t += __shfl_xor_sync(0xffffffffu, t, 1);
+            if ((tid & 31) == 0) s_e[tid >> 5][j] = t;
+        }
+        __syncthreads();
+        if (tid < 12) {
+            double t = 0.0;
+#pragma unroll
+            for (int w = 0; w < 8; w++) t += (double)s_e[w][tid];
+            if (t != 0.0) atomicAdd(dL_dE + tid, t);
+        }
+    }
     if (!own) return;
     if (exposure) {
 #pragma unroll
@@ -230,6 +261,25 @@ post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const flo
 #pragma unroll
         for (int k = 0; k < 3; k++) dL_dimg[(size_t)k * plane + p] = g[k];
     }
+}
+
+// One thread: the eight status words of train_single's step (h3dgs/singlestep.py) -- loss, photometric loss, L1, SSIM,
+// pure inverse-depth L1, D, longest tile list, binning overflow -- and the exposure gradient in fp32 for the caller's
+// optimizer, zero for an overflowed frame (which contributes no gradient anywhere else either).
+__global__ void single_step_status_kernel(const double* __restrict__ sums, const double* __restrict__ depth_sum,
+                                          const float* __restrict__ depth_weight, double inv_numel, double inv_pixels,
+                                          double lambda_dssim, const uint32_t* __restrict__ scan_info,
+                                          const double* __restrict__ dL_dE, float* __restrict__ exposure_grad, double* __restrict__ out)
+{
+    if (exposure_grad)
+        for (int j = 0; j < 12; j++) exposure_grad[j] = scan_info[2] ? 0.f : (float)dL_dE[j];
+    const double l1 = sums[0] * inv_numel, ssim = sums[1] * inv_numel;
+    const double photo = (1.0 - lambda_dssim) * l1 + lambda_dssim * (1.0 - ssim);
+    // weight 0: the term is absent, as train_single.py:111 skips it
+    const double w = depth_sum ? (double)*depth_weight : 0.0, depth = w != 0.0 ? *depth_sum * inv_pixels : 0.0;
+    out[0] = photo + w * depth;
+    out[1] = photo; out[2] = l1; out[3] = ssim; out[4] = depth;
+    out[5] = (double)scan_info[0]; out[6] = (double)scan_info[1]; out[7] = (double)scan_info[2];
 }
 
 // One thread: the eight status words of the post-loss step (h3dgs/poststep.py) -- loss, L1, SSIM, rows the cut needs, D,
@@ -300,8 +350,33 @@ extern "C" int h3dgs_post_loss_backward(int32_t H, int32_t W, const float* img, 
     if (H <= 0 || W <= 0 || !img || !gt || !maps || !coeffs || !dL_dimg) { set_error("post_loss_backward: bad arguments"); return H3DGS_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
     const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 1);
-    post_loss_backward_kernel<<<grid, 256, 0, s>>>(H, W, img, gt, exposure, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, make_loss_window());
+    post_loss_backward_kernel<false><<<grid, 256, 0, s>>>(H, W, img, gt, exposure, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, nullptr, make_loss_window());
     H3_LAUNCHED("post_loss_backward", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_post_loss_backward_exposure(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure,
+                                                 const float* mask, const float* maps, const float* coeffs, float* dL_dimg,
+                                                 double* dL_dexposure, void* stream)
+{
+    if (H <= 0 || W <= 0 || !img || !gt || !maps || !coeffs || !dL_dimg || !dL_dexposure) { set_error("post_loss_backward_exposure: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    H3_CUDA(cudaMemsetAsync(dL_dexposure, 0, 12 * sizeof(double), s));
+    const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 1);
+    ProfScope prof(H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, s);
+    post_loss_backward_kernel<true><<<grid, 256, 0, s>>>(H, W, img, gt, exposure, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, dL_dexposure, make_loss_window());
+    H3_LAUNCHED("post_loss_backward_exposure", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_single_step_status(const double* sums, const double* depth_sum, const float* depth_weight, double inv_numel,
+                                        double inv_pixels, double lambda_dssim, const uint32_t* scan_info,
+                                        const double* dL_dexposure, float* exposure_grad, double* out, void* stream)
+{
+    if (!sums || !scan_info || !out || (depth_sum && !depth_weight) || (exposure_grad && !dL_dexposure)) { set_error("single_step_status: NULL argument"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    single_step_status_kernel<<<1, 1, 0, s>>>(sums, depth_sum, depth_weight, inv_numel, inv_pixels, lambda_dssim, scan_info, dL_dexposure, exposure_grad, out);
+    H3_LAUNCHED("single_step_status", 0, s);
     return H3DGS_OK;
 }
 

@@ -27,6 +27,7 @@ EXPORTS = [
     "h3dgs_knn_scratch_bytes", "h3dgs_dist_knn3", "h3dgs_build_hierarchy_scratch_bytes", "h3dgs_build_hierarchy",
     "h3dgs_merge_hierarchies_scratch_bytes", "h3dgs_merge_hierarchies",
     "h3dgs_post_loss_forward", "h3dgs_post_loss_backward", "h3dgs_post_step_status",
+    "h3dgs_post_loss_backward_exposure", "h3dgs_invdepth_l1_grad", "h3dgs_densify_stats", "h3dgs_single_step_status",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -146,6 +147,14 @@ def bind(l):
         l.h3dgs_post_step_status.restype = C.c_int
         l.h3dgs_post_step_status.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int32, C.c_int32,
                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        l.h3dgs_post_loss_backward_exposure.restype = C.c_int
+        l.h3dgs_post_loss_backward_exposure.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 9
+        l.h3dgs_single_step_status.restype = C.c_int
+        l.h3dgs_single_step_status.argtypes = [C.c_void_p] * 3 + [C.c_double] * 3 + [C.c_void_p] * 5
+    l.h3dgs_invdepth_l1_grad.restype = C.c_int
+    l.h3dgs_invdepth_l1_grad.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
+    l.h3dgs_densify_stats.restype = C.c_int
+    l.h3dgs_densify_stats.argtypes = [C.c_int32] + [C.c_void_p] * 7
     if hasattr(l, "h3dgs_sparse_adam"):          # sparse Adam (absent from the emulation build)
         l.h3dgs_sparse_adam.restype = C.c_int
         l.h3dgs_sparse_adam.argtypes = [C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -178,7 +187,7 @@ def launch_count():
     return int(lib().h3dgs_launch_count())
 
 
-STAGES = 13
+STAGES = 16
 
 
 def profile_enable(on=True):

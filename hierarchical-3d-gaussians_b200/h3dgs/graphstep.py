@@ -53,7 +53,175 @@ def _check_index_sizing(n_nodes, rows):
                          "index arrays of one entry per node")
 
 
-class GraphedStep:
+class GraphedBase:
+    """What a sync-free step needs whatever it renders: the state-buffer callback of the C-ABI, the scan_info view, the
+    two-slot target upload, capture of graph A and of graph B once per slot, and replay.  A subclass provides dev, P, W, H,
+    bin_capacity, gt_bufs, status_dev, _part_a() and _part_b(slot), and calls _init_replay() from its constructor."""
+
+    def _init_replay(self):
+        dev = self.dev
+        self._bufs = [None, None, None]
+        self._alloc_cb = _lib.ALLOC_FN(self._alloc)     # keep the callback object alive
+        self._scan_info = None
+        self.graph_a = self.graph_b = None
+        self.launches_per_step = 0
+        self._upload_slot, self._pending = 0, None      # slot the next upload_target() writes; (slot, event) of an upload not yet consumed
+        self._done = torch.cuda.Event()                 # recorded after part B of every step
+        self._done.record(torch.cuda.current_stream(dev))
+        self._slot_done = [torch.cuda.Event(), torch.cuda.Event()]      # recorded after the part B that read slot k: it may be overwritten
+        for e in self._slot_done:
+            e.record(torch.cuda.current_stream(dev))
+
+    # ---- C-ABI plumbing -------------------------------------------------------------------
+    def _alloc(self, _user, which, nbytes):
+        t = self._bufs[which]
+        if t is None or t.numel() < nbytes:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("state buffer grew during capture: run one eager step first")
+            t = torch.empty((max(int(nbytes), 1),), dtype=torch.uint8, device=self.dev)
+            self._bufs[which] = t
+        return t.data_ptr()
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.dev).cuda_stream
+
+    def scan_info(self):
+        """int32 view [D, longest tile list, overflow] inside the image state."""
+        if self._scan_info is None:
+            v = _lib.StateView()
+            b = self._bufs
+            _lib.check(self.L.h3dgs_state_layout(self.P, self.W, self.H, self.bin_capacity, b[0].data_ptr(),
+                                                 b[1].data_ptr(), b[2].data_ptr(), C.byref(v)))
+            off = v.scan_info - b[2].data_ptr()
+            self._scan_info = b[2][off:off + 12].view(torch.int32)
+        return self._scan_info
+
+    def n_contrib_view(self):
+        """int32 view [H*W] of the per-pixel last-contributor index inside the image state (bench bookkeeping:
+        its sum is the number of list positions the classic per-pixel formulation walks)."""
+        v = _lib.StateView()
+        b = self._bufs
+        _lib.check(self.L.h3dgs_state_layout(self.P, self.W, self.H, self.bin_capacity, b[0].data_ptr(),
+                                             b[1].data_ptr(), b[2].data_ptr(), C.byref(v)))
+        off = v.n_contrib - b[2].data_ptr()
+        return b[2][off:off + 4 * self.W * self.H].view(torch.int32)
+
+    # ---- driving --------------------------------------------------------------------------
+    def set_camera(self, cam):
+        """cam: pipeline.DeviceCamera (device tensors) -- three small device copies."""
+        self.view.copy_(cam.viewmatrix.reshape(16), non_blocking=True)
+        self.proj.copy_(cam.projmatrix.reshape(16), non_blocking=True)
+        self.campos.copy_(cam.campos.reshape(3), non_blocking=True)
+
+    def _set_mask(self, slot, mask):
+        """the alpha mask of target slot `slot` ([1,H,W] or [H,W]; None = ones, as the reference's loader falls back to);
+        for steps that keep mask_bufs, one plane per slot or None when built without a mask"""
+        if self.mask_bufs[slot] is None:
+            if mask is not None:
+                raise ValueError("this step was built without a mask (mask=False)")
+        elif mask is None:
+            self.mask_bufs[slot].fill_(1.0)
+        else:
+            self.mask_bufs[slot].copy_(mask.reshape(self.H, self.W), non_blocking=True)
+
+    def _set_exposure(self, exposure):
+        """this step's [3,4] (or larger: its top 3x4 block) exposure; None = identity, as the renderers do for an image
+        without one; for steps that keep `exposure` (a device [3,4], or None when built without) and `_identity`"""
+        if self.exposure is not None:
+            self.exposure.copy_(self._identity if exposure is None else exposure.detach()[:3, :4], non_blocking=True)
+        elif exposure is not None:
+            raise ValueError("this step was built without an exposure (exposure=False)")
+
+    def _raster_args(self, tanfovx, tanfovy, do_depth=0):
+        """h3dgs_raster_args of the whole frame on one GPU, flat: P rows of the scene's arrays, capacity mode"""
+        sc = self.scene
+        a = _lib.RasterArgs()
+        a.P, a.sh_degree, a.sh_coeffs = self.P, self.sh_degree, int(sc.shs.shape[1])
+        a.image_width, a.image_height = self.W, self.H
+        a.tanfovx, a.tanfovy, a.scale_modifier = float(tanfovx), float(tanfovy), 1.0
+        a.prefiltered, a.debug, a.do_depth = 0, 0, int(do_depth)
+        a.bg, a.viewmatrix, a.projmatrix, a.campos = _ptr(self.bg), _ptr(self.view), _ptr(self.proj), _ptr(self.campos)
+        a.means3D, a.shs, a.colors_precomp, a.opacities = _ptr(sc.means3D), _ptr(sc.shs), None, _ptr(sc.opacities)
+        a.scales, a.rotations, a.cov3D_precomp = _ptr(sc.scales), _ptr(sc.rotations), None
+        a.shard_count, a.shard_index = 1, 0
+        a.bin_capacity, a.sort_capacity = self.bin_capacity, self.sort_capacity
+        return a
+
+    def _fill_slot(self, slot, src):
+        """what travels with a target into its slot (subclasses add the target's mask, depth maps, ...)"""
+        self.gt_bufs[slot].copy_(src, non_blocking=True)
+
+    def upload_target(self, src, stream, *with_target, **kw):
+        """Copy the NEXT step's target (device tensor or pinned host tensor) into one of the two static target slots on
+        `stream`, after the last step that read that slot has finished; returns the event to hand to step() as gt_ready
+        (step() also picks the slot up by itself).  With two slots the copy overlaps the whole step that is still running
+        (and this step's graph A).  with_target: what a subclass keeps beside the target in the slot."""
+        slot = self._upload_slot
+        self._upload_slot ^= 1
+        with torch.cuda.stream(stream):
+            stream.wait_event(self._slot_done[slot])
+            self._fill_slot(slot, src, *with_target, **kw)
+            ready = torch.cuda.Event()
+            ready.record(stream)
+        self._pending = (slot, ready)
+        return ready
+
+    def _warm_up(self):
+        """the eager step before the capture, on whatever the input buffers hold.  Its outputs are overwritten by the
+        first real step; a subclass whose step accumulates into state that outlives a step keeps that state out of it"""
+        self._part_a(); self._part_b(0)
+
+    def capture(self):
+        """One eager step (sizes the state buffers, creates the library's side stream), then capture: graph A, and graph B
+        once per target buffer."""
+        s = torch.cuda.Stream(self.dev)
+        s.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(s):
+            self._warm_up()
+        torch.cuda.current_stream(self.dev).wait_stream(s)
+        torch.cuda.synchronize(self.dev)
+        l0 = _lib.launch_count()
+        self.graph_a = torch.cuda.CUDAGraph()
+        self.graph_b = [torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()]
+        with torch.cuda.graph(self.graph_a):
+            self._part_a()
+        with torch.cuda.graph(self.graph_b[0], pool=self.graph_a.pool()):
+            self._part_b(0)
+        self.launches_per_step = _lib.launch_count() - l0      # library kernels inside one replay of A + B
+        with torch.cuda.graph(self.graph_b[1], pool=self.graph_a.pool()):
+            self._part_b(1)
+
+    def step(self, cam=None, gt=None, gt_ready=None):
+        """cam/gt: optional new inputs (copied into the static buffers; gt goes into buffer 0).  gt_ready: the event
+        upload_target() returned, when the caller uploads the target on another stream: this step then reads the buffer
+        that upload wrote."""
+        if cam is not None:
+            self.set_camera(cam)
+        slot = 0
+        if gt is not None:
+            self.gt_bufs[0].copy_(gt, non_blocking=True)
+            self._pending = None
+        elif self._pending is not None:
+            slot, ev = self._pending
+            self._pending = None
+            gt_ready = ev if gt_ready is None else gt_ready
+        cur = torch.cuda.current_stream(self.dev)
+        if self.graph_a is None:
+            self._part_a()
+            if gt_ready is not None:
+                cur.wait_event(gt_ready)
+            self._part_b(slot)
+        else:
+            self.graph_a.replay()
+            if gt_ready is not None:
+                cur.wait_event(gt_ready)
+            self.graph_b[slot].replay()
+        self._done.record(cur)
+        self._slot_done[slot].record(cur)
+        return self.status_dev
+
+
+class GraphedStep(GraphedBase):
     """scene: pipeline.Scene with a hierarchy.  The camera-independent sizes (W, H, tanfov) are fixed per
     instance (launch constants inside the graphs); camera, target and LOD threshold are device-resident
     inputs that change between replays (set_camera, upload_target / step(gt=), set_threshold)."""
@@ -90,7 +258,6 @@ class GraphedStep:
         # step instead of only its graph A; graph B is captured once per buffer.  self.gt is buffer 0 (gs.gt.copy_ / step(gt=))
         self.gt_bufs = [f(3, H, W), f(3, H, W)]
         self.gt = self.gt_bufs[0]
-        self._upload_slot, self._pending = 0, None          # buffer the next upload_target() writes; (slot, event) of an upload not yet consumed
         self.threshold_dev = torch.full((1,), self.threshold, dtype=torch.float32, device=dev)   # read by the cut kernels
         # static outputs
         self.count = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -125,45 +292,18 @@ class GraphedStep:
             self.accum = torch.zeros(max(world * chunk, 1) * 10, dtype=torch.float32, device=dev)
         self.lod_scratch = torch.empty(int(self.L.h3dgs_expand_scratch_bytes(self.N_nodes)), dtype=torch.uint8, device=dev)
         self.sky_arange = torch.arange(self.S, dtype=torch.int64, device=dev)
-        self._bufs = [None, None, None]
-        self._alloc_cb = _lib.ALLOC_FN(self._alloc)     # keep the callback object alive
+        self._init_replay()
         self.args = self._make_args(tanfovx, tanfovy)
-        self._scan_info = None
-        self.graph_a = self.graph_b = None
-        self.launches_per_step = 0
-        self._done = torch.cuda.Event()                 # recorded after part B of every step
-        self._done.record(torch.cuda.current_stream(dev))
-        self._slot_done = [torch.cuda.Event(), torch.cuda.Event()]      # recorded after the part B that read buffer k: it may be overwritten
-        for e in self._slot_done:
-            e.record(torch.cuda.current_stream(dev))
         if capture:
             self.capture()
 
-    # ---- C-ABI plumbing -------------------------------------------------------------------
-    def _alloc(self, _user, which, nbytes):
-        t = self._bufs[which]
-        if t is None or t.numel() < nbytes:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("state buffer grew during capture: run one eager step first")
-            t = torch.empty((max(int(nbytes), 1),), dtype=torch.uint8, device=self.dev)
-            self._bufs[which] = t
-        return t.data_ptr()
-
     def _make_args(self, tanfovx, tanfovy):
         sc = self.scene
-        a = _lib.RasterArgs()
-        a.P, a.sh_degree, a.sh_coeffs = self.P, self.sh_degree, int(sc.shs.shape[1])
-        a.image_width, a.image_height = self.W, self.H
-        a.tanfovx, a.tanfovy, a.scale_modifier = float(tanfovx), float(tanfovy), 1.0
-        a.prefiltered, a.debug, a.do_depth = 0, 0, 0
-        a.bg, a.viewmatrix, a.projmatrix, a.campos = _ptr(self.bg), _ptr(self.view), _ptr(self.proj), _ptr(self.campos)
-        a.means3D, a.shs, a.colors_precomp, a.opacities = _ptr(sc.means3D), _ptr(sc.shs), None, _ptr(sc.opacities)
-        a.scales, a.rotations, a.cov3D_precomp = _ptr(sc.scales), _ptr(sc.rotations), None
+        a = self._raster_args(tanfovx, tanfovy)
         a.interpolation_weights, a.num_node_kids = _ptr(sc.interpolation_weights), _ptr(sc.num_siblings)
         a.render_indices, a.parent_indices, a.num_source = _ptr(sc.render_indices), _ptr(sc.parent_indices), self.N
         a.shard_count, a.shard_index = self.world, self.rank
         a.grad_row_begin, a.grad_row_end = hdist.row_block(self.P, self.world, self.rank) if (self.world > 1 and not self.peer) else (0, 0)
-        a.bin_capacity, a.sort_capacity = self.bin_capacity, self.sort_capacity
         if self.peer:
             a.peer_count, a.grad_cyclic_log2 = self.world, self.cyclic_log2
             for r in range(self.world):
@@ -171,9 +311,6 @@ class GraphedStep:
                 a.peer_image[r] = self.arena.ptr("image", r) if r == self.rank else None
                 a.peer_stage[r] = self.arena.ptr("stage", r)
         return a
-
-    def _stream(self):
-        return torch.cuda.current_stream(self.dev).cuda_stream
 
     # ---- the two halves of the step (eager or under capture) ------------------------------
     def _part_a(self):
@@ -247,101 +384,10 @@ class GraphedStep:
         _lib.check(L.h3dgs_step_status(self.loss_sum.data_ptr(), 1.0 / numel, self.count.data_ptr(), self.S, self.P,
                                        self.scan_info().data_ptr(), 1 if self.peer else 0, self.status_dev.data_ptr(), self._stream()))
 
-    def scan_info(self):
-        """int32 view [D, longest tile list, overflow] inside the image state."""
-        if self._scan_info is None:
-            v = _lib.StateView()
-            b = self._bufs
-            _lib.check(self.L.h3dgs_state_layout(self.P, self.W, self.H, self.bin_capacity, b[0].data_ptr(),
-                                                 b[1].data_ptr(), b[2].data_ptr(), C.byref(v)))
-            off = v.scan_info - b[2].data_ptr()
-            self._scan_info = b[2][off:off + 12].view(torch.int32)
-        return self._scan_info
-
-    def n_contrib_view(self):
-        """int32 view [H*W] of the per-pixel last-contributor index inside the image state (bench bookkeeping:
-        its sum is the number of list positions the classic per-pixel formulation walks)."""
-        v = _lib.StateView()
-        b = self._bufs
-        _lib.check(self.L.h3dgs_state_layout(self.P, self.W, self.H, self.bin_capacity, b[0].data_ptr(),
-                                             b[1].data_ptr(), b[2].data_ptr(), C.byref(v)))
-        off = v.n_contrib - b[2].data_ptr()
-        return b[2][off:off + 4 * self.W * self.H].view(torch.int32)
-
-    # ---- driving --------------------------------------------------------------------------
-    def set_camera(self, cam):
-        """cam: pipeline.DeviceCamera (device tensors) -- three small device copies."""
-        self.view.copy_(cam.viewmatrix.reshape(16), non_blocking=True)
-        self.proj.copy_(cam.projmatrix.reshape(16), non_blocking=True)
-        self.campos.copy_(cam.campos.reshape(3), non_blocking=True)
-
     def set_threshold(self, threshold):
         """A new LOD threshold for the next step (train_post.py:66-74 draws one per step)."""
         self.threshold = float(threshold)
         self.threshold_dev.fill_(self.threshold)
-
-    def upload_target(self, src, stream):
-        """Copy the NEXT step's target (device tensor or pinned host tensor) into one of the two static target buffers on
-        `stream`, after the last step that read that buffer has finished; returns the event to hand to step() as gt_ready.
-        With two buffers the copy overlaps the whole step that is still running (and this step's graph A)."""
-        slot = self._upload_slot
-        self._upload_slot ^= 1
-        with torch.cuda.stream(stream):
-            stream.wait_event(self._slot_done[slot])
-            self.gt_bufs[slot].copy_(src, non_blocking=True)
-            ready = torch.cuda.Event()
-            ready.record(stream)
-        self._pending = (slot, ready)
-        return ready
-
-    def capture(self):
-        """One eager step (sizes the state buffers, creates the library's side stream), then capture: graph A, and graph B
-        once per target buffer."""
-        s = torch.cuda.Stream(self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s):
-            self._part_a(); self._part_b(0)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        l0 = _lib.launch_count()
-        self.graph_a = torch.cuda.CUDAGraph()
-        self.graph_b = [torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()]
-        with torch.cuda.graph(self.graph_a):
-            self._part_a()
-        with torch.cuda.graph(self.graph_b[0], pool=self.graph_a.pool()):
-            self._part_b(0)
-        self.launches_per_step = _lib.launch_count() - l0      # library kernels inside one replay of A + B
-        with torch.cuda.graph(self.graph_b[1], pool=self.graph_a.pool()):
-            self._part_b(1)
-
-    def step(self, cam=None, gt=None, gt_ready=None):
-        """cam/gt: optional new inputs (copied into the static buffers; gt goes into buffer 0).  gt_ready: the event
-        upload_target() returned, when the caller uploads the target on another stream: this step then reads the buffer
-        that upload wrote."""
-        if cam is not None:
-            self.set_camera(cam)
-        slot = 0
-        if gt is not None:
-            self.gt_bufs[0].copy_(gt, non_blocking=True)
-            self._pending = None
-        elif self._pending is not None:
-            slot, ev = self._pending
-            self._pending = None
-            gt_ready = ev if gt_ready is None else gt_ready
-        cur = torch.cuda.current_stream(self.dev)
-        if self.graph_a is None:
-            self._part_a()
-            if gt_ready is not None:
-                cur.wait_event(gt_ready)
-            self._part_b(slot)
-        else:
-            self.graph_a.replay()
-            if gt_ready is not None:
-                cur.wait_event(gt_ready)
-            self.graph_b[slot].replay()
-        self._done.record(cur)
-        self._slot_done[slot].record(cur)
-        return self.status_dev
 
     def status(self):
         """One 48-byte read-back: loss, rows needed, D, longest tile list, overflow flags."""

@@ -6,7 +6,8 @@ size_average=True) combined as in train_post.py:134-140:
     loss = (1 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1 - ssim(image, gt))
 
 but one CUDA kernel forward and one backward instead of 5 grouped conv2d + ~20 elementwise kernels and
-their autograd.  Gradients flow to `image` only (the ground truth is data).  No CPU fallback.
+their autograd.  Gradients flow to `image` only (the ground truth is data); `single_loss`, train_single's objective,
+also has them to the trained exposure and the inverse depth.  No CPU fallback.
 """
 
 import torch
@@ -159,3 +160,105 @@ def post_loss(image, gt, lambda_dssim=0.2, exposure=None, mask=None):
     None (all ones).  One CUDA kernel forward and one backward; gradient to `image` only (pretrained exposures are
     frozen, the mask is data)."""
     return _PostLoss.apply(image, gt, lambda_dssim, exposure, mask)
+
+
+class _SingleLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, image, invdepth, exposure, gt, lambda_dssim, mask, mono_invdepth, depth_mask, depth_weight):
+        from diff_gaussian_rasterization._C import _on_device
+        if not _on_device(image):
+            raise RuntimeError("single_loss needs CUDA tensors (there is no CPU fallback)")
+        img = image.detach().float().contiguous()
+        ref = gt.detach().float().contiguous()
+        if img.dim() != 3 or img.shape[0] != 3 or img.shape != ref.shape:
+            raise RuntimeError("expected image and gt of identical shape [3,H,W]")
+        _, H, W = img.shape
+        dev = img.device
+        E = exposure_block(exposure, dev)
+        M = mask_plane(mask, H, W, dev)
+        L = _lib.lib()
+        sums = torch.empty(2, dtype=torch.float64, device=dev)
+        maps = torch.empty((3, 3, H, W), dtype=torch.float32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        depth = mono_invdepth is not None
+        with torch.cuda.device(dev):
+            _lib.check(L.h3dgs_post_loss_forward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(E), _ptr(M), sums.data_ptr(),
+                                                 maps.data_ptr(), st))
+            if depth:
+                if invdepth is None or invdepth.numel() != H * W:
+                    raise RuntimeError("the depth term needs the rasterizer's inverse depth [1,H,W] (do_depth=True)")
+                inv = invdepth.detach().float().contiguous()
+                mono = mask_plane(mono_invdepth, H, W, dev)
+                dmask = mask_plane(depth_mask, H, W, dev) if depth_mask is not None else torch.ones((H, W), device=dev)
+                w = torch.as_tensor(depth_weight, dtype=torch.float32, device=dev).reshape(())
+                dsum = torch.empty(1, dtype=torch.float64, device=dev)
+                dinv = torch.empty((H, W), dtype=torch.float32, device=dev)
+                _lib.check(L.h3dgs_invdepth_l1_grad(H, W, inv.data_ptr(), mono.data_ptr(), dmask.data_ptr(), w.data_ptr(),
+                                                    dinv.data_ptr(), dsum.data_ptr(), st))
+        n = float(img.numel())
+        l1, ssim = sums[0] / n, sums[1] / n
+        lam = float(lambda_dssim)
+        photo = (1.0 - lam) * l1 + lam * (1.0 - ssim)
+        if depth:
+            depth_l1 = dsum[0] / float(H * W)
+            loss = photo + w.double() * depth_l1
+            ctx.dinv = dinv                     # dL/dinvdepth for an upstream gradient of 1 to the loss
+        else:
+            depth_l1, loss, ctx.dinv = torch.zeros((), dtype=torch.float64, device=dev), photo, None
+        ctx.save_for_backward(img, ref, maps)
+        ctx.E, ctx.M, ctx.lam, ctx.n = E, M, lam, n
+        ctx.in_shape = image.shape
+        ctx.inv_shape = None if invdepth is None else invdepth.shape
+        ctx.exposure_like = exposure if (exposure is not None and ctx.needs_input_grad[2]) else None
+        depth_l1 = depth_l1.float()
+        ctx.mark_non_differentiable(depth_l1)       # reported, as Ll1depth_pure is; its gradient travels through the loss
+        return loss.float(), photo.float(), l1.float(), ssim.float(), depth_l1
+
+    @staticmethod
+    def backward(ctx, g_loss, g_photo, g_l1, g_ssim, _g_depth):
+        img, ref, maps = ctx.saved_tensors
+        _, H, W = img.shape
+        dev = img.device
+        L = _lib.lib()
+        st = torch.cuda.current_stream(dev).cuda_stream
+        coeffs = _coefficients(g_loss + g_photo, g_l1, g_ssim, ctx.lam, ctx.n)
+        grad = torch.empty_like(img)
+        g_inv = g_E = None
+        with torch.cuda.device(dev):
+            if ctx.exposure_like is not None:
+                dE = torch.empty((3, 4), dtype=torch.float64, device=dev)
+                _lib.check(L.h3dgs_post_loss_backward_exposure(H, W, img.data_ptr(), ref.data_ptr(), _ptr(ctx.E), _ptr(ctx.M),
+                                                               maps.data_ptr(), coeffs.data_ptr(), grad.data_ptr(),
+                                                               dE.data_ptr(), st))
+                g_E = torch.zeros_like(ctx.exposure_like)
+                g_E[:3, :4] = dE.to(g_E.dtype)
+            else:
+                _lib.check(L.h3dgs_post_loss_backward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(ctx.E), _ptr(ctx.M),
+                                                      maps.data_ptr(), coeffs.data_ptr(), grad.data_ptr(), st))
+            if ctx.dinv is not None and ctx.needs_input_grad[1]:
+                # the forward's one pass wrote the gradient with the term's sum; times 1 under loss.backward(): exact
+                g_inv = (ctx.dinv * g_loss.float()).view(ctx.inv_shape)
+            elif ctx.needs_input_grad[1]:
+                g_inv = torch.zeros(ctx.inv_shape, dtype=torch.float32, device=dev)
+        return grad.view(ctx.in_shape), g_inv, g_E, None, None, None, None, None, None
+
+
+def single_loss(image, invdepth, gt, lambda_dssim=0.2, exposure=None, mask=None, mono_invdepth=None, depth_mask=None,
+                depth_weight=0.0):
+    """train_single's objective on the raw rasterizer outputs `image` [3,H,W] and `invdepth` [1,H,W]
+    -> (loss, photo, l1, ssim, depth_l1) scalars:
+
+        a     = clamp(image.permute(1,2,0) @ E[:3,:3] + E[:3,3], 0, 1) * mask     (render() :115-118, train_single.py:102-104)
+        photo = (1-l) * mean|a - gt| + l * (1 - SSIM(a, gt))                       (train_single.py:106-108)
+        depth_l1 = mean|(invdepth - mono_invdepth) * depth_mask|                   (:115, Ll1depth_pure)
+        loss  = photo + depth_weight * depth_l1
+
+    exposure: the image's trained [3,4] or [4,4] exposure (None = identity); when it requires grad it receives its
+    gradient in its own shape, zero outside the top 3x4 block.  The depth term is absent when mono_invdepth is None or
+    depth_weight is the number 0 (train_single.py:111: the weight schedule reached 0, or the view's depth is
+    unreliable); depth_weight may be a device tensor.  Gradients go to image, invdepth and exposure; gt, the masks and
+    the mono depth are data; depth_l1 is a reported value (Ll1depth_pure), not differentiable on its own.  One CUDA
+    kernel forward and one backward for the photometric term, and one pass for the depth term and its gradient."""
+    if mono_invdepth is not None and not torch.is_tensor(depth_weight) and float(depth_weight) == 0.0:
+        mono_invdepth = None
+    return _SingleLoss.apply(image, invdepth, exposure, gt, lambda_dssim, mask, mono_invdepth, depth_mask, depth_weight)

@@ -114,14 +114,17 @@ def _skybox_weights(scene, n):
         scene.num_siblings[n:n + S] = 1
 
 
-def render_flat(scene, cam, bg, sh_degree=3):
-    """`render()` of the reference minus exposure/clamp (flat chunk training, config #2)."""
-    rs = make_settings(scene, cam, bg, sh_degree)
-    means2D = torch.zeros_like(scene.means3D, requires_grad=scene.means3D.requires_grad)
-    img, radii, _ = GaussianRasterizer(rs)(means3D=scene.means3D, means2D=means2D, shs=scene.shs, colors_precomp=None,
-                                           opacities=scene.opacities, scales=scene.scales, rotations=scene.rotations,
-                                           cov3D_precomp=None)
-    return img, radii
+def render_flat(scene, cam, bg, sh_degree=3, do_depth=False, means2D=None):
+    """`render()` of the reference minus exposure/clamp (flat chunk training, config #2) -> (img, radii), and with
+    do_depth=True (as render() sets it, :57) -> (img, radii, invdepth [1,H,W]).  means2D: the caller's [N,3] sink for the
+    screen-space gradient (render()'s viewspace_points); None makes one."""
+    rs = make_settings(scene, cam, bg, sh_degree, do_depth=do_depth)
+    if means2D is None:
+        means2D = torch.zeros_like(scene.means3D, requires_grad=scene.means3D.requires_grad)
+    img, radii, invdepth = GaussianRasterizer(rs)(means3D=scene.means3D, means2D=means2D, shs=scene.shs, colors_precomp=None,
+                                                  opacities=scene.opacities, scales=scene.scales, rotations=scene.rotations,
+                                                  cov3D_precomp=None)
+    return (img, radii, invdepth) if do_depth else (img, radii)
 
 
 def render_hier(scene, cam, bg, threshold, sh_degree=3):
@@ -195,6 +198,53 @@ def post_step(scene, cam, bg, gt, threshold, lambda_dssim=0.2, exposure=None, ma
     loss, l1, ssim = post_loss(img, gt, lambda_dssim, exposure, mask)
     loss.backward()
     return (loss, l1, ssim), radii, n
+
+
+class DensifyStats:
+    """The three per-Gaussian tensors train_single's densification reads (scene/gaussian_model.py: max_radii2D [N],
+    xyz_gradient_accum [N,1], denom [N,1]), zero for a new model."""
+
+    def __init__(self, N, device="cuda"):
+        self.max_radii2D = torch.zeros(N, device=device)
+        self.xyz_gradient_accum = torch.zeros((N, 1), device=device)
+        self.denom = torch.zeros((N, 1), device=device)
+
+    def update(self, radii, d_means2D, scan_info=None):
+        """train_single.py:147-148 in one kernel (h3dgs_densify_stats).  scan_info: the state word of a capacity-mode
+        frame (an overflowed frame then changes nothing); None = the exact mode."""
+        from . import _lib
+        P = self.denom.shape[0]
+        if radii.shape != (P,) or radii.dtype != torch.int32 or not radii.is_contiguous():
+            raise ValueError(f"radii must be a contiguous int32 [{P}] (the statistics hold {P} rows), not {radii.dtype} {tuple(radii.shape)}")
+        if d_means2D.shape != (P, 3) or d_means2D.dtype != torch.float32 or not d_means2D.is_contiguous():
+            raise ValueError(f"d_means2D must be a contiguous float32 [{P}, 3], not {d_means2D.dtype} {tuple(d_means2D.shape)}")
+        with torch.cuda.device(radii.device):
+            _lib.check(_lib.lib().h3dgs_densify_stats(radii.shape[0], radii.data_ptr(), d_means2D.data_ptr(),
+                                                     self.max_radii2D.data_ptr(), self.xyz_gradient_accum.data_ptr(),
+                                                     self.denom.data_ptr(), None if scan_info is None else scan_info.data_ptr(),
+                                                     torch.cuda.current_stream().cuda_stream))
+
+
+def single_step(scene, cam, bg, gt, lambda_dssim=0.2, exposure=None, mask=None, mono_invdepth=None, depth_mask=None,
+                depth_weight=0.0, stats=None, sh_degree=3):
+    """One step of train_single's loop body (train_single.py:94-148) on a flat scene, on the exact path: render() with
+    do_depth, the objective (h3dgs.loss.single_loss: exposure, clamp, alpha mask, (1-l) L1 + l (1 - SSIM), plus
+    depth_weight times the inverse-depth L1 when mono_invdepth is given and the weight is not 0), backward, and the
+    densification statistics into `stats` (a DensifyStats; None skips them).  Gradients land in the scene's tensors and,
+    when `exposure` requires grad, in exposure.grad.  Also the path that re-runs a frame
+    h3dgs.singlestep.GraphedSingleStep flagged as overflowed.
+    -> ((loss, photo, l1, ssim, depth_l1) device scalars, radii, means2D with its .grad)"""
+    from .loss import single_loss
+    if scene.hier:
+        raise ValueError("single_step trains a flat scene (train_single.py); a hierarchy goes through post_step")
+    scene.zero_grad()
+    means2D = torch.zeros_like(scene.means3D, requires_grad=True)
+    img, radii, invdepth = render_flat(scene, cam, bg, sh_degree, do_depth=True, means2D=means2D)
+    out = single_loss(img, invdepth, gt, lambda_dssim, exposure, mask, mono_invdepth, depth_mask, depth_weight)
+    out[0].backward()
+    if stats is not None:
+        stats.update(radii, means2D.grad)
+    return out, radii, means2D
 
 
 def fov_threshold(tau, cam):

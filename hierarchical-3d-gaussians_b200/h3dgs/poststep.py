@@ -76,30 +76,10 @@ class GraphedPostStep(GraphedStep):
                                             self.count.data_ptr(), self.S, self.P, self.scan_info().data_ptr(),
                                             self.status_dev.data_ptr(), st))
 
-    def _set_mask(self, slot, mask):
-        if self.mask_bufs[slot] is None:
-            if mask is not None:
-                raise ValueError("this step was built without a mask (mask=False)")
-            return
-        if mask is None:
-            self.mask_bufs[slot].fill_(1.0)               # no alpha mask: ones, as the reference's loader falls back to
-        else:
-            self.mask_bufs[slot].copy_(mask.reshape(self.H, self.W), non_blocking=True)
-
-    def upload_target(self, src, stream, mask=None):
-        """Copy the NEXT step's target and its alpha mask ([1,H,W] or [H,W]; None = ones) into one of the two target slots
-        on `stream`, after the last step that read that slot has finished; returns the event to hand to step() as
-        gt_ready (step() also picks the slot up by itself)."""
-        slot = self._upload_slot
-        self._upload_slot ^= 1
-        with torch.cuda.stream(stream):
-            stream.wait_event(self._slot_done[slot])
-            self.gt_bufs[slot].copy_(src, non_blocking=True)
-            self._set_mask(slot, mask)
-            ready = torch.cuda.Event()
-            ready.record(stream)
-        self._pending = (slot, ready)
-        return ready
+    def _fill_slot(self, slot, src, mask=None):
+        """upload_target(src, stream, mask): the NEXT step's target and its alpha mask ([1,H,W] or [H,W]; None = ones)"""
+        self.gt_bufs[slot].copy_(src, non_blocking=True)
+        self._set_mask(slot, mask)
 
     def step(self, cam=None, gt=None, mask=None, exposure=None, gt_ready=None):
         """cam, gt (+ its mask; None = ones): optional new inputs, copied into the static buffers (the target into slot
@@ -107,10 +87,7 @@ class GraphedPostStep(GraphedStep):
         an image without one.  gt_ready: the event upload_target() returned."""
         if mask is not None and gt is None:
             raise ValueError("a mask travels with its target: pass gt with it, or upload both with upload_target")
-        if self.exposure is not None:
-            self.exposure.copy_(self._identity if exposure is None else exposure[:3, :4], non_blocking=True)
-        elif exposure is not None:
-            raise ValueError("this step was built without an exposure (exposure=False)")
+        self._set_exposure(exposure)
         if gt is not None:
             self._set_mask(0, mask)
         return super().step(cam, gt, gt_ready)

@@ -266,7 +266,8 @@ int h3dgs_l1_ssim_backward(int32_t C, int32_t H, int32_t W, const float* img, co
  *          (ds/dmu1, ds/dE11, ds/dE12 at a) are written when non-NULL (needed by backward).
  * backward: dL/dy_c = [0 <= y_c <= 1] * mask * (coeffs[0] sign(a_c - gt_c) + coeffs[1] d(sum ssim)/d a_c),
  *          dL_dimg_k = (E[k][0] dL/dy_0 + E[k][1] dL/dy_1) + E[k][2] dL/dy_2 (or dL/dy_k without exposure); coeffs is a
- *          DEVICE pointer to two floats.  There is no gradient to the exposure or the mask.
+ *          DEVICE pointer to two floats.  There is no gradient to the mask, and none to the exposure here (train_post's
+ *          exposures are frozen; h3dgs_post_loss_backward_exposure has it).
  * With exposure and mask NULL and img in [0, 1] both equal h3dgs_l1_ssim_forward / _backward with C = 3, bit for bit.
  * Nothing synchronises with the host: exposure and mask may change between replays of a CUDA graph. */
 int h3dgs_post_loss_forward(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure, const float* mask,
@@ -279,6 +280,46 @@ int h3dgs_post_loss_backward(int32_t H, int32_t W, const float* img, const float
  * row_capacity. */
 int h3dgs_post_step_status(const double* sums, double inv_numel, double lambda_dssim, const int32_t* count, int32_t extra_rows,
                            int32_t row_capacity, const uint32_t* scan_info, double* out, void* stream);
+
+/* ---- train_single's objective (train_single.py:97-117, 147-148 on render()'s exposure and clamp, gaussian_renderer/__init__.py:115-118).
+ * Its photometric forward is h3dgs_post_loss_forward.  In train_single the exposure is a trained parameter, so its
+ * backward is h3dgs_post_loss_backward with one more output: dL_dexposure, a DEVICE [3][4] of doubles (zeroed here),
+ *   dL/dE[k][c] = sum over pixels of img_k * dL/dy_c  (k, c < 3),   dL/dE[c][3] = sum over pixels of dL/dy_c,
+ * the gradient with respect to the identity when exposure is NULL.  Order: each img_k * dL/dy_c is one rounded fp32
+ * product; the terms of a 16x16 pixel tile (pixels outside the frame count as 0) are summed per warp by an xor butterfly
+ * (offsets 16, 8, 4, 2, 1) in fp32, the eight warp sums of the tile are added in warp order in fp64, and the tiles are
+ * added by fp64 atomics in arrival order.  The same kernel as h3dgs_post_loss_backward, in the same pass over the image:
+ * dL_dimg is that function's bit for bit. */
+int h3dgs_post_loss_backward_exposure(int32_t H, int32_t W, const float* img, const float* gt, const float* exposure,
+                                      const float* mask, const float* maps, const float* coeffs, float* dL_dimg,
+                                      double* dL_dexposure, void* stream);
+/* The inverse-depth term (train_single.py:111-117) and its gradient in one pass.  invdepth, mono, depth_mask,
+ * dL_dinvdepth: [H,W]; weight: a DEVICE float (depth_l1_weight(iteration): it may change between replays of a graph).
+ *   t = (invdepth - mono) * depth_mask (difference, then product, each rounded), *sum [device double, zeroed here] =
+ *   sum |t| (unweighted: Ll1depth_pure times H W), dL_dinvdepth = ((weight / (H W)) * sign(t)) * depth_mask with
+ *   sign(0) = 0 as torch.abs; weight 0 writes zeros. */
+int h3dgs_invdepth_l1_grad(int32_t H, int32_t W, const float* invdepth, const float* mono, const float* depth_mask,
+                           const float* weight, float* dL_dinvdepth, double* sum, void* stream);
+/* Densification statistics of one step (train_single.py:147, scene/gaussian_model.py:687-689), for the rows with
+ * radii > 0 (the others are untouched):
+ *   max_radii2D[i] = max(max_radii2D[i], (float)radii[i]);  xyz_gradient_accum[i] = max(n, xyz_gradient_accum[i]) with
+ *   n = sqrtf(x*x + y*y) of dL_dmeans2D[i] ([P,3]; both products, the sum and the root rounded to fp32, no FMA);
+ *   denom[i] += 1.  The maxima propagate NaN as torch.max.
+ * scan_info (h3dgs_state_view.scan_info of a capacity-mode frame) or NULL: when scan_info[2] is set nothing is changed --
+ * an overflowed frame has the radii of the real frame but zero gradients, and the caller re-runs it in exact mode. */
+int h3dgs_densify_stats(int32_t P, const int32_t* radii, const float* dL_dmeans2D, float* max_radii2D,
+                        float* xyz_gradient_accum, float* denom, const uint32_t* scan_info, void* stream);
+/* Status words of the sync-free train_single step, written by one device thread: out[0] = loss = photo + weight * depth,
+ * out[1] = photo = (1 - lambda) L1 + lambda (1 - SSIM), out[2] = L1 = sums[0] * inv_numel, out[3] = SSIM = sums[1] *
+ * inv_numel, out[4] = depth = *depth_sum * inv_pixels (Ll1depth_pure; 0 and no depth term when depth_sum is NULL or
+ * the weight is 0, as train_single.py:111 skips it),
+ * out[5..7] = scan_info[0..2] (D, longest tile list, binning overflow).  depth_weight: the device float of
+ * h3dgs_invdepth_l1_grad.  exposure_grad (optional, DEVICE float [3][4]) receives dL_dexposure rounded to fp32 for the
+ * exposure's optimizer, or zeros when scan_info[2] is set: an overflowed frame renders the background only, and like
+ * its Gaussian gradients its exposure gradient must not reach an optimizer. */
+int h3dgs_single_step_status(const double* sums, const double* depth_sum, const float* depth_weight, double inv_numel,
+                             double inv_pixels, double lambda_dssim, const uint32_t* scan_info, const double* dL_dexposure,
+                             float* exposure_grad, double* out, void* stream);
 
 /* L1 loss and its gradient in one pass (the loss of bench.py's step; train_post.py:134-142 with lambda_dssim = 0):
  * *loss_sum [device double, zeroed here] = sum |img - gt|, dL_dimg = sign(img - gt) * scale (scale = 1 / numel for the
@@ -435,6 +476,7 @@ enum {
     H3DGS_STAGE_PREPROCESS = 0, H3DGS_STAGE_SCAN, H3DGS_STAGE_DUPLICATE, H3DGS_STAGE_SORT, H3DGS_STAGE_RANGES,
     H3DGS_STAGE_GATHER, H3DGS_STAGE_RENDER_FWD, H3DGS_STAGE_RENDER_BWD, H3DGS_STAGE_PREPROCESS_BWD,
     H3DGS_STAGE_LOD_CUT, H3DGS_STAGE_LOD_WEIGHTS, H3DGS_STAGE_PREPROCESS_COLOR, H3DGS_STAGE_SH_BACKWARD,
+    H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, H3DGS_STAGE_INVDEPTH_L1, H3DGS_STAGE_DENSIFY_STATS,
     H3DGS_STAGE_COUNT
 };
 int h3dgs_profile_enable(int on);
