@@ -46,10 +46,8 @@ duplicate_with_keys_kernel(int P, int W, int H, int shard_count, int shard_index
     const float4 a = records[i].a;
     const float ix = a.x, iy = a.y;
     const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-    const int rminx = min(gx, max(0, (int)((ix - rad) / kTile)));
-    const int rminy = min(gy, max(0, (int)((iy - rad) / kTile)));
-    const int rmaxx = min(gx, max(0, (int)((ix + rad + kTile - 1) / kTile)));
-    const int rmaxy = min(gy, max(0, (int)((iy + rad + kTile - 1) / kTile)));
+    const TileRect rect = tile_rect(ix, iy, rad, gx, gy);
+    const int rminx = rect.x, rminy = rect.y, rmaxx = rect.z, rmaxy = rect.w;
     uint32_t off = (i == 0) ? 0u : offsets[i - 1];
     const uint32_t dbits = __float_as_uint(depths[i]);
     for (int y = rminy; y < rmaxy; y++) {
@@ -187,10 +185,8 @@ emit_to_tiles_kernel(int P, int W, int H, int shard_count, int shard_index, cons
     const float4 a = records[i].a;
     const float ix = a.x, iy = a.y;
     const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-    const int rminx = min(gx, max(0, (int)((ix - rad) / kTile)));
-    const int rminy = min(gy, max(0, (int)((iy - rad) / kTile)));
-    const int rmaxx = min(gx, max(0, (int)((ix + rad + kTile - 1) / kTile)));
-    const int rmaxy = min(gy, max(0, (int)((iy + rad + kTile - 1) / kTile)));
+    const TileRect rect = tile_rect(ix, iy, rad, gx, gy);
+    const int rminx = rect.x, rminy = rect.y, rmaxx = rect.z, rmaxy = rect.w;
     const uint32_t dbits = __float_as_uint(depths[i]);
     // The slot claims return a value, so each costs a full L2 round trip: walk the rect as a flat index
     // and keep four independent claims (then four range loads, then four stores) in flight per thread.

@@ -40,6 +40,33 @@ static_assert(sizeof(Record) == 48, "record must be 48 bytes");
 
 __host__ __device__ inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// float -> int toward zero, saturating at INT_MIN / INT_MAX, NaN -> 0 (DESIGN.md §7).  On the device this is what a
+// cast compiles to (cvt.rzi.s32.f32); in C++ the cast is undefined out of range, so host builds of these sources
+// (and oracle.c) spell the saturation out.
+__device__ __forceinline__ int f2i_sat(float x) {
+#ifdef __CUDA_ARCH__
+    return __float2int_rz(x);
+#else
+    if (!(x == x)) return 0;
+    if (x >= 2147483648.0f) return 2147483647;
+    if (x <= -2147483648.0f) return -2147483647 - 1;
+    return (int)x;
+#endif
+}
+__device__ __forceinline__ bool is_finite(float x) { return (x - x) == 0.0f; }
+
+// Tile rect [x, z) x [y, w) of a splat with pixel centre (ix, iy) and integer radius: K1 takes it, the binning
+// kernels re-derive it from the stored centre and radius, so the three must be one expression.
+struct TileRect { int x, y, z, w; };
+__device__ __forceinline__ TileRect tile_rect(float ix, float iy, int rad, int gx, int gy) {
+    TileRect r;
+    r.x = min(gx, max(0, f2i_sat((ix - rad) / kTile)));
+    r.y = min(gy, max(0, f2i_sat((iy - rad) / kTile)));
+    r.z = min(gx, max(0, f2i_sat((ix + rad + kTile - 1) / kTile)));
+    r.w = min(gy, max(0, f2i_sat((iy + rad + kTile - 1) / kTile)));
+    return r;
+}
+
 // ---- state buffer layouts (byte offsets inside the three alloc'd buffers) ----
 struct GeomLayout {
     size_t depths, tiles_touched, offsets, rank_mask, records, scan_temp, total;

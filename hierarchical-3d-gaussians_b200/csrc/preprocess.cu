@@ -154,13 +154,16 @@ preprocess_kernel(int P, const float* __restrict__ means3D, const float* __restr
             const float my_radius = ceilf(3.f * sqrtf(fmaxf(l1, l2)));
             const float ix = ((ndcx + 1.0f) * W - 1.0f) * 0.5f;
             const float iy = ((ndcy + 1.0f) * H - 1.0f) * 0.5f;
-            const int rad = (int)my_radius;
+            const int rad = f2i_sat(my_radius);
             const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-            const int rminx = min(gx, max(0, (int)((ix - rad) / kTile)));
-            const int rminy = min(gy, max(0, (int)((iy - rad) / kTile)));
-            const int rmaxx = min(gx, max(0, (int)((ix + rad + kTile - 1) / kTile)));
-            const int rmaxy = min(gy, max(0, (int)((iy + rad + kTile - 1) / kTile)));
-            const int area = (rmaxx - rminx) * (rmaxy - rminy);
+            const TileRect rect = tile_rect(ix, iy, rad, gx, gy);
+            const int rminx = rect.x, rminy = rect.y, rmaxx = rect.z, rmaxy = rect.w;
+            // A row that does not project to finite values (a NaN or overflowing parameter) or whose radius is not
+            // positive is invisible, like an empty rect: the binning kernels skip radii <= 0, so a row that counted
+            // tiles here with such a radius would leave histogram slots that nobody fills.
+            const bool projects = rad > 0 && is_finite(my_radius) && is_finite(vz) && is_finite(ix) && is_finite(iy)
+                               && is_finite(conx) && is_finite(cony) && is_finite(conz);
+            const int area = projects ? (rmaxx - rminx) * (rmaxy - rminy) : 0;
             if (area != 0) {
                 // colour: precomputed colours are copied here; SH colours are filled in by
                 // preprocess_color_kernel (separate launch: keeps this kernel at high occupancy)

@@ -162,6 +162,16 @@ static void sh_to_rgb(int deg, int M, f3 pos, const float* campos, const float* 
     }
 }
 
+/* float -> int toward zero, saturating, NaN -> 0: the device's conversion, which the C cast leaves undefined
+ * out of range (DESIGN.md 7) */
+static int f2i_sat(float x) {
+    if (!(x == x)) return 0;
+    if (x >= 2147483648.0f) return 2147483647;
+    if (x <= -2147483648.0f) return -2147483647 - 1;
+    return (int)x;
+}
+static int is_finite(float x) { return (x - x) == 0.0f; }
+
 /* ------------------------------------------------------------------ */
 /* K1: per-Gaussian preprocess                                         */
 /* ------------------------------------------------------------------ */
@@ -205,12 +215,15 @@ void oracle_preprocess(int P, int deg, int M,
         float my_radius = ceilf(3.f * sqrtf(fmaxf(l1, l2)));
         float ix = ((px + 1.0f) * W - 1.0f) * 0.5f;
         float iy = ((py + 1.0f) * H - 1.0f) * 0.5f;
-        int r = (int)my_radius;
-        int rminx = (int)((ix - r) / TILE), rminy = (int)((iy - r) / TILE);
-        int rmaxx = (int)((ix + r + TILE - 1) / TILE), rmaxy = (int)((iy + r + TILE - 1) / TILE);
+        int r = f2i_sat(my_radius);
+        int rminx = f2i_sat((ix - r) / TILE), rminy = f2i_sat((iy - r) / TILE);
+        int rmaxx = f2i_sat((ix + r + TILE - 1) / TILE), rmaxy = f2i_sat((iy + r + TILE - 1) / TILE);
         rminx = rminx < 0 ? 0 : (rminx > gx ? gx : rminx); rminy = rminy < 0 ? 0 : (rminy > gy ? gy : rminy);
         rmaxx = rmaxx < 0 ? 0 : (rmaxx > gx ? gx : rmaxx); rmaxy = rmaxy < 0 ? 0 : (rmaxy > gy ? gy : rmaxy);
         if ((rmaxx - rminx) * (rmaxy - rminy) == 0) continue;
+        /* a row that does not project to finite values, or whose radius is not positive, is invisible */
+        if (!(r > 0 && is_finite(my_radius) && is_finite(pv.z) && is_finite(ix) && is_finite(iy)
+              && is_finite(conic[0]) && is_finite(conic[1]) && is_finite(conic[2]))) continue;
 
         if (colors_precomp) { for (int k = 0; k < 3; k++) rgb[3 * i + k] = colors_precomp[3 * i + k]; }
         else sh_to_rgb(deg, M, p, campos, shs + (size_t)i * M * 3, rgb + 3 * i, clamped + 3 * i);

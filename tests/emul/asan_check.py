@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE ONLY.  A memcheck for the kernels without a GPU: build the emulation library with
 AddressSanitizer (heap and globals -- `__shared__` arrays are globals in the emulator; stack instrumentation is off
 because the fibers switch stacks by hand), preload libasan so that numpy's buffers get red zones too, and run a set
-of scenes through both blend variants, the sharded schedule, the fused cut gather and the device-side LOD cut /
-capacity mode.  Usage:   python tests/emul/asan_check.py          (re-executes itself under LD_PRELOAD)
+of scenes through both blend variants, the sharded schedule, the fused cut gather, the device-side LOD cut /
+capacity mode, and the preprocess edge families with non-finite inputs and huge splats (tests/preprocess_ref.py).  Usage:   python tests/emul/asan_check.py          (re-executes itself under LD_PRELOAD)
 A deliberately short output buffer is reported as heap-buffer-overflow (checked by --negative-control)."""
 import os
 import subprocess
@@ -53,7 +53,18 @@ def run_cases(so, negative):
         print("negative control: NOT reported")
         return
     import test_emu_kernels_cpu as T
+    import preprocess_ref as PR
+    import test_preprocess_ref_cpu as TP
     n = 0
+    # rows that do not project to finite values (NaN / inf in each input) and huge splats (saturated radius and rect):
+    # the binning must never be handed a counted tile that no row fills
+    for which in PR.NONFINITE_INPUTS:
+        TP.test_rows_that_do_not_project_are_invisible(emu, which)
+        n += 1
+    TP.hold(emu, PR.family_huge())
+    TP.hold(emu, PR.family_degenerate())
+    n += 2
+    print(f"asan: {n} non-finite / huge / degenerate cases done", flush=True)
     for gw in ("0", "1"):
         os.environ["H3DGS_GROUPWALK"] = gw
         for (P, W, H, kw, depth) in [(3000, 256, 192, dict(mode="hier", seed=42), True), (1500, 160, 96, dict(seed=7), False),

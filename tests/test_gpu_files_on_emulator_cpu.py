@@ -15,7 +15,7 @@ def test_gpu_parity_files_pass_on_the_emulator():
     env = dict(os.environ, H3DGS_EMULATE="1")
     r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_parity.py", "tests/test_gpu_hierarchy.py",
                         "tests/test_gpu_pipeline.py", "tests/test_gpu_blend_edges.py",
-                        "tests/test_gpu_chain_edges.py", "-q", "-p", "no:cacheprovider",
+                        "tests/test_gpu_chain_edges.py", "tests/test_gpu_preprocess_edges.py", "-q", "-p", "no:cacheprovider",
                         "-k", "not 3840 and not full_size and not config2"],
                        cwd=ROOT, env=env, capture_output=True, text=True, timeout=1500)
     tail = r.stdout[-1500:]
