@@ -183,6 +183,11 @@ def check(rc):
     return rc
 
 
+def ptr(t):
+    """a tensor as a pointer argument: NULL for None and for an empty tensor"""
+    return None if (t is None or t.numel() == 0) else t.data_ptr()
+
+
 def launch_count():
     return int(lib().h3dgs_launch_count())
 

@@ -5,7 +5,7 @@ The drop-in flow of render_hierarchy.py pays, per frame, two host round trips (t
 sizing the binning buffer), a .cpu() of the camera centre, ~25 PyTorch kernels of gather and lerp, the exposure matmul,
 clamps, crop, mask and the metric reductions with a syncing .double() each.  Here one graph per camera size holds
 
-  * h3dgs_lod_cut with the threshold read on the device, and the skybox rows after the cut (GraphedStep._part_a);
+  * h3dgs_lod_cut with the threshold read on the device, and the skybox rows after the cut (graphstep.GraphedLodCut);
   * the capacity-mode forward with the cut gather and lerp fused into K1;
   * h3dgs_eval_metrics (csrc/metrics.cu): exposure, clamp, train_test_exp crop, alpha mask, per-channel squared error
     and the SSIM map sum in one pass, and a one-thread finisher that stores [psnr, ssim, status words] at a slot taken
@@ -20,20 +20,21 @@ import numpy as np
 import torch
 
 from . import _lib, pipeline
-from .graphstep import GraphedStep, _check_index_sizing, _ptr
+from ._lib import ptr
+from .graphstep import GraphedLodCut
 
 
 def _metrics(L, H, W, image, gt, exposure, mask, x0, out_image, sums, counter, results, stream, count=None, extra_rows=0,
              row_capacity=0, scan_info=None):
-    _lib.check(L.h3dgs_eval_metrics(H, W, image.data_ptr(), gt.data_ptr(), _ptr(exposure), _ptr(mask), x0, _ptr(out_image),
-                                    sums.data_ptr(), _ptr(count), extra_rows, row_capacity, _ptr(scan_info),
+    _lib.check(L.h3dgs_eval_metrics(H, W, image.data_ptr(), gt.data_ptr(), ptr(exposure), ptr(mask), x0, ptr(out_image),
+                                    sums.data_ptr(), ptr(count), extra_rows, row_capacity, ptr(scan_info),
                                     counter.data_ptr(), results.data_ptr(), results.shape[0], stream))
 
 
-class GraphedRender(GraphedStep):
+class GraphedRender(GraphedLodCut):
     """Forward-only counterpart of GraphedStep for hierarchy scenes on one GPU: ONE graph = LOD cut (device threshold) +
-    skybox rows + capacity-mode forward + metrics pass.  It reuses GraphedStep's plumbing (state buffers, raster
-    arguments, _part_a, set_camera, set_threshold, scan_info) and allocates no gradient buffers.
+    skybox rows + capacity-mode forward + metrics pass.  It shares GraphedStep's plumbing (state buffers, raster
+    arguments, the LOD cut, set_camera, set_threshold, scan_info, capture) and allocates no gradient buffers.
 
     W, H, tanfovx, tanfovy are fixed per instance, and so are whether an exposure and a mask are applied and the
     train_test_exp crop.  Inputs that change between replays: set_camera, set_threshold, and the static buffers
@@ -44,91 +45,50 @@ class GraphedRender(GraphedStep):
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None, bin_capacity=1 << 22,
                  sort_capacity=4096, exposure=False, mask=False, train_test_exp=False, keep_image=False, results=None,
                  counter=None, max_frames=1024, capture=True):
-        if not scene.hier:
-            raise ValueError("GraphedRender drives the hierarchy path (LOD cut + fused gather/lerp)")
-        self.L = _lib.lib()
-        self.scene, self.W, self.H = scene, int(W), int(H)
-        self.threshold, self.sh_degree = float(threshold), int(sh_degree)
-        self.world, self.rank, self.group, self.peer, self.arena = 1, 0, None, False, None
-        dev = scene.means3D.device
-        self.dev = dev
-        self.N = scene.means3D.shape[0]
-        self.N_nodes = scene.nodes.shape[0]
-        _check_index_sizing(self.N_nodes, self.N)
-        self.S = scene.skybox_points
-        self.P = int(row_capacity) if row_capacity else self.N
-        if not (0 < self.P <= self.N):
-            raise ValueError(f"row_capacity must be in (0, {self.N}]")
-        self.bin_capacity, self.sort_capacity = int(bin_capacity), int(sort_capacity)
-        f = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
-        self.view, self.proj, self.campos = f(16), f(16), f(3)
-        self.bg = bg.to(dev).float().contiguous()
-        self.threshold_dev = torch.full((1,), self.threshold, dtype=torch.float32, device=dev)
-        self.count = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.radii = torch.zeros(self.P, dtype=torch.int32, device=dev)
-        self.image = f(3, H, W)
-        self.gt = f(3, H, W)
-        self.exposure = torch.eye(3, 4, device=dev) if exposure else None
-        self.mask = torch.ones((H, W), device=dev) if mask else None
-        self.x0 = self.W // 2 if train_test_exp else 0
-        self.out_image = f(3, H, self.W - self.x0) if keep_image else None
+        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity)
+        dev, H, W = self.dev, self.H, self.W
+        self.image = self._zeros(3, H, W)
+        self._init_inputs(exposure, mask)
+        self.x0 = W // 2 if train_test_exp else 0
+        self.out_image = self._zeros(3, H, W - self.x0) if keep_image else None
         self.sums = torch.zeros(4, dtype=torch.float64, device=dev)
         self.results = results if results is not None else torch.zeros((max_frames, _lib.EVAL_ROW), dtype=torch.float64, device=dev)
         self.counter = counter if counter is not None else torch.zeros(1, dtype=torch.int32, device=dev)
         self._warm_counter = torch.zeros(1, dtype=torch.int32, device=dev)          # the eager frame before capture
         self._warm_results = torch.zeros((1, _lib.EVAL_ROW), dtype=torch.float64, device=dev)
-        self.lod_scratch = torch.empty(int(self.L.h3dgs_expand_scratch_bytes(self.N_nodes)), dtype=torch.uint8, device=dev)
-        self.sky_arange = torch.arange(self.S, dtype=torch.int64, device=dev)
-        self._bufs = [None, None, None]
-        self._alloc_cb = _lib.ALLOC_FN(self._alloc)
-        self.args = self._make_args(tanfovx, tanfovy)
-        self._scan_info = None
-        self.graph = None
-        self.launches_per_frame = 0
+        self.args = self._raster_args(tanfovx, tanfovy)
         if capture:
             self.capture()
 
-    def _part_eval(self, counter, results):
-        _metrics(self.L, self.H, self.W, self.image, self.gt, self.exposure, self.mask, self.x0, self.out_image, self.sums,
-                 counter, results, self._stream(), count=self.count, extra_rows=self.S, row_capacity=self.P,
-                 scan_info=self.scan_info())
+    graph = property(lambda self: self.graph_a)                         # the frame's one graph
+    launches_per_frame = property(lambda self: self.launches_per_step)
 
-    def capture(self):
-        """One eager frame (sizes the state buffers; its row goes to a private slot), then capture of the single graph."""
-        s = torch.cuda.Stream(self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s):
-            self._part_a()
-            self._part_eval(self._warm_counter, self._warm_results)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        l0 = _lib.launch_count()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._part_a()
-            self._part_eval(self.counter, self.results)
-        self.launches_per_frame = _lib.launch_count() - l0
+    def _part_a(self, counter=None, results=None):
+        """LOD cut -> forward -> metrics pass, whose row goes to slot counter++ of results"""
+        self._cut()
+        self._forward(self.image)
+        _metrics(self.L, self.H, self.W, self.image, self.gt, self.exposure, self.mask, self.x0, self.out_image, self.sums,
+                 self.counter if counter is None else counter, self.results if results is None else results, self._stream(),
+                 count=self.count, extra_rows=self.S, row_capacity=self.P, scan_info=self.scan_info())
+
+    def _warm_up(self):
+        """capture()'s eager frame (sizes the state buffers): its row goes to a private slot"""
+        self._part_a(self._warm_counter, self._warm_results)
 
     def set_inputs(self, gt=None, mask=None, exposure=None):
-        """Copy a frame's target [3,H,W], mask ([1,H,W] or [H,W]) and exposure [3,4] (or larger: the top 3x4 block; None =
-        identity) into the static buffers.  Device or pinned host tensors: nothing here waits for the host."""
+        """Copy a frame's target [3,H,W], mask ([1,H,W] or [H,W]; None = ones) and exposure [3,4] (or larger: the top 3x4
+        block; None = identity) into the static buffers.  Device or pinned host tensors: nothing here waits for the host."""
         if gt is not None:
             self.gt.copy_(gt, non_blocking=True)
-        if mask is not None and self.mask is not None:
-            self.mask.copy_(mask.reshape(self.H, self.W), non_blocking=True)
-        if self.exposure is not None:
-            if exposure is None:
-                self.exposure.copy_(torch.eye(3, 4, device=self.dev))
-            else:
-                self.exposure.copy_(exposure[:3, :4], non_blocking=True)
+        self._set_mask(0, mask)
+        self._set_exposure(exposure)
 
     def frame(self):
         """Render and evaluate one frame with the current inputs: a graph replay (eager when not captured)."""
-        if self.graph is None:
+        if self.graph_a is None:
             self._part_a()
-            self._part_eval(self.counter, self.results)
         else:
-            self.graph.replay()
+            self.graph_a.replay()
 
 
 def _stage(t):
@@ -241,7 +201,8 @@ class HierarchyEvaluator:
         results = torch.zeros((1, _lib.EVAL_ROW), dtype=torch.float64, device=self.dev)
         out = torch.zeros((3, cam.H, cam.W - r.x0), device=self.dev) if self.keep_images else None
         gt = self.targets[ci].to(self.dev)
-        mask = None if self.masks is None else self.masks[ci].to(self.dev).reshape(cam.H, cam.W).contiguous()
+        mask = None if self.masks is None else self.masks[ci]      # None: no mask, the same as ones
+        mask = None if mask is None else mask.to(self.dev).reshape(cam.H, cam.W).contiguous()
         E = None
         if self.exposures is not None:
             E = torch.eye(3, 4, device=self.dev) if self.exposures[ci] is None else self.exposures[ci][:3, :4].contiguous()
@@ -278,10 +239,10 @@ def evaluate_hierarchy(scene, cameras, targets, taus, masks=None, exposures=None
     """The evaluation of render_hierarchy.py (render_set for every tau), sync-free.
 
     scene: pipeline.Scene with a hierarchy; cameras: pipeline.DeviceCamera per test view; targets: [3,H,W] per camera
-    (device, or host: pinned here); masks: [1,H,W] alpha masks per camera or None; exposures: [3,4] per camera (None
-    entries = no exposure for that camera, as render_post does for a missing one) or None; train_test_exp: evaluate the
-    right half only; capacities: dict(row_capacity, bin_capacity, sort_capacity) instead of the learned ones.
-    Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
+    (device, or host: pinned here); masks: [1,H,W] alpha masks per camera (None entries = ones, the reference loader's
+    fallback) or None; exposures: [3,4] per camera (None entries = no exposure for that camera, as render_post does for
+    a missing one) or None; train_test_exp: evaluate the right half only; capacities: dict(row_capacity, bin_capacity,
+    sort_capacity) instead of the learned ones.  Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
     -> see HierarchyEvaluator.finish."""
     ev = HierarchyEvaluator(scene, cameras, targets, taus, masks, exposures, train_test_exp, keep_images, bg, sh_degree,
                             capacities)

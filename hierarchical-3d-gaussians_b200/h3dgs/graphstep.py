@@ -39,10 +39,8 @@ import torch.distributed as dist
 
 from . import _lib
 from . import dist as hdist
-
-
-def _ptr(t):
-    return None if (t is None or t.numel() == 0) else t.data_ptr()
+from ._lib import ptr
+from .loss import _coefficients
 
 
 def _check_index_sizing(n_nodes, rows):
@@ -54,12 +52,31 @@ def _check_index_sizing(n_nodes, rows):
 
 
 class GraphedBase:
-    """What a sync-free step needs whatever it renders: the state-buffer callback of the C-ABI, the scan_info view, the
-    two-slot target upload, capture of graph A and of graph B once per slot, and replay.  A subclass provides dev, P, W, H,
-    bin_capacity, gt_bufs, status_dev, _part_a() and _part_b(slot), and calls _init_replay() from its constructor."""
+    """What every sync-free form shares whatever it renders: the library handle, the sizes and capacities, the camera
+    buffers, the state-buffer callback of the C-ABI, the scan_info view, the flat raster arguments, the two target slots
+    with what travels with a target, the forward and backward launches, train_post's objective, capture and replay.
 
-    def _init_replay(self):
-        dev = self.dev
+    A subclass provides _part_a() and, when the form has a second graph, _part_b(slot); it sets `args` (_raster_args) and
+    status_dev, and allocates what it renders into (image; _init_grads, _init_inputs, _init_post_loss)."""
+    exposure, mask_bufs, dinvdepth = None, (None, None), None       # forms without an exposure, a mask, a depth term
+    _part_b = None                                                  # forms without a part B: one graph
+
+    def __init__(self, scene, W, H, sh_degree, row_capacity, bin_capacity, sort_capacity):
+        self.L = _lib.lib()
+        self.scene, self.W, self.H, self.sh_degree = scene, int(W), int(H), int(sh_degree)
+        dev = self.dev = scene.means3D.device
+        N = self.N = scene.means3D.shape[0]                 # rows of the parameter arrays (hierarchy + skybox)
+        self.P = int(row_capacity) if row_capacity else N
+        if not (0 < self.P <= N):
+            raise ValueError(f"row_capacity must be in (0, {N}]")
+        self.bin_capacity, self.sort_capacity = int(bin_capacity), int(sort_capacity)
+        f = self._zeros
+        self.view, self.proj, self.campos = f(16), f(16), f(3)
+        # two target buffers: the upload of the next step's target (25 MB over PCIe, ~1 ms) then overlaps the WHOLE current
+        # step instead of only its graph A; graph B is captured once per buffer.  self.gt is buffer 0 (gs.gt.copy_ / step(gt=))
+        self.gt_bufs = [f(3, self.H, self.W), f(3, self.H, self.W)]
+        self.gt = self.gt_bufs[0]
+        self.radii = torch.zeros(self.P, dtype=torch.int32, device=dev)
         self._bufs = [None, None, None]
         self._alloc_cb = _lib.ALLOC_FN(self._alloc)     # keep the callback object alive
         self._scan_info = None
@@ -71,6 +88,38 @@ class GraphedBase:
         self._slot_done = [torch.cuda.Event(), torch.cuda.Event()]      # recorded after the part B that read slot k: it may be overwritten
         for e in self._slot_done:
             e.record(torch.cuda.current_stream(dev))
+
+    def _zeros(self, *shape):
+        return torch.zeros(shape, dtype=torch.float32, device=self.dev)
+
+    def _init_inputs(self, exposure, mask):
+        """the exposure (a device [3,4], identity until set) and one alpha-mask plane per target slot (all ones until set),
+        for a form built to apply them"""
+        self._identity = torch.eye(3, 4, device=self.dev)
+        self.exposure = self._identity.clone() if exposure else None
+        self.mask_bufs = [torch.ones((self.H, self.W), device=self.dev) for _ in range(2)] if mask else [None, None]
+        self.mask = self.mask_bufs[0]
+
+    def _init_grads(self, accum_rows):
+        """what the backward reads and writes: dL/dimage (dcolor), the full-size Gaussian gradients, d_means2D and the
+        [accum_rows, 10] accumulator of the per-tile replay"""
+        f, N = self._zeros, self.N
+        self.dcolor = f(3, self.H, self.W)
+        self.grads = dict(means3D=f(N, 3), shs=f(N, self.scene.shs.shape[1], 3), opacities=f(N, 1), scales=f(N, 3),
+                          rotations=f(N, 4))
+        self.d_means2D = f(self.P, 3)
+        self.accum = torch.zeros(max(accum_rows, 1) * 10, dtype=torch.float32, device=self.dev)
+
+    def _init_post_loss(self, lambda_dssim, exposure, mask):
+        """train_post's objective (csrc/loss.cu's post-loss kernels): the exposure, the mask slots, the sums and derivative
+        maps, and the weights of sign(a - gt) and of the SSIM-sum gradient for loss.backward(), formed as the exact path's
+        backward (loss.post_loss / single_loss) forms them, so that the graphed dL/dimage equals the eager one bit for bit"""
+        self._init_inputs(exposure, mask)
+        self.lambda_dssim = float(lambda_dssim)
+        self.sums = torch.zeros(2, dtype=torch.float64, device=self.dev)
+        self.maps = self._zeros(3, 3, self.H, self.W)
+        one, zero = torch.ones((), device=self.dev), torch.zeros((), device=self.dev)
+        self.coeffs = _coefficients(one, zero, zero, self.lambda_dssim, float(3 * self.H * self.W))
 
     # ---- C-ABI plumbing -------------------------------------------------------------------
     def _alloc(self, _user, which, nbytes):
@@ -106,6 +155,51 @@ class GraphedBase:
         off = v.n_contrib - b[2].data_ptr()
         return b[2][off:off + 4 * self.W * self.H].view(torch.int32)
 
+    def _raster_args(self, tanfovx, tanfovy, do_depth=0):
+        """h3dgs_raster_args of the whole frame on one GPU, flat: P rows of the scene's arrays, capacity mode"""
+        sc = self.scene
+        a = _lib.RasterArgs()
+        a.P, a.sh_degree, a.sh_coeffs = self.P, self.sh_degree, int(sc.shs.shape[1])
+        a.image_width, a.image_height = self.W, self.H
+        a.tanfovx, a.tanfovy, a.scale_modifier = float(tanfovx), float(tanfovy), 1.0
+        a.prefiltered, a.debug, a.do_depth = 0, 0, int(do_depth)
+        a.bg, a.viewmatrix, a.projmatrix, a.campos = ptr(self.bg), ptr(self.view), ptr(self.proj), ptr(self.campos)
+        a.means3D, a.shs, a.colors_precomp, a.opacities = ptr(sc.means3D), ptr(sc.shs), None, ptr(sc.opacities)
+        a.scales, a.rotations, a.cov3D_precomp = ptr(sc.scales), ptr(sc.rotations), None
+        a.shard_count, a.shard_index = 1, 0
+        a.bin_capacity, a.sort_capacity = self.bin_capacity, self.sort_capacity
+        return a
+
+    # ---- launches shared by the forms (eager or under capture) ----------------------------
+    def _forward(self, out, invdepth=None):
+        """capacity-mode forward into `out` (None: the peer form's image, see GraphedStep) and `invdepth`"""
+        n = C.c_int64(0)
+        _lib.check(self.L.h3dgs_rasterize_forward(C.byref(self.args), self._alloc_cb, None, ptr(out), self.radii.data_ptr(),
+                                                  ptr(invdepth), C.byref(n), self._stream()))
+
+    def _post_loss(self, slot, exposure_grad=None):
+        """train_post's objective against target slot `slot` and its mask: sums, derivative maps and dL/dimage (dcolor);
+        with exposure_grad (a device fp64 [3,4]), also dL/dE from the same pass"""
+        L, st = self.L, self._stream()
+        args = (self.H, self.W, self.image.data_ptr(), self.gt_bufs[slot].data_ptr(), ptr(self.exposure),
+                ptr(self.mask_bufs[slot]))
+        _lib.check(L.h3dgs_post_loss_forward(*args, self.sums.data_ptr(), self.maps.data_ptr(), st))
+        args += (self.maps.data_ptr(), self.coeffs.data_ptr(), self.dcolor.data_ptr())
+        if exposure_grad is None:
+            _lib.check(L.h3dgs_post_loss_backward(*args, st))
+        else:
+            _lib.check(L.h3dgs_post_loss_backward_exposure(*args, exposure_grad.data_ptr(), st))
+
+    def _backward(self, phases):
+        """h3dgs_rasterize_backward from dcolor (and dinvdepth when the form has it) into grads, d_means2D and accum;
+        phases as include/h3dgs.h defines them (3 = the whole backward)"""
+        g, b = self.grads, self._bufs
+        _lib.check(self.L.h3dgs_rasterize_backward(
+            C.byref(self.args), self.radii.data_ptr(), b[0].data_ptr(), b[1].data_ptr(), b[2].data_ptr(), self.bin_capacity,
+            self.dcolor.data_ptr(), ptr(self.dinvdepth), g["means3D"].data_ptr(), self.d_means2D.data_ptr(),
+            g["shs"].data_ptr(), None, g["opacities"].data_ptr(), g["scales"].data_ptr(), g["rotations"].data_ptr(), None,
+            self.accum.data_ptr(), phases, self._stream()))
+
     # ---- driving --------------------------------------------------------------------------
     def set_camera(self, cam):
         """cam: pipeline.DeviceCamera (device tensors) -- three small device copies."""
@@ -114,8 +208,7 @@ class GraphedBase:
         self.campos.copy_(cam.campos.reshape(3), non_blocking=True)
 
     def _set_mask(self, slot, mask):
-        """the alpha mask of target slot `slot` ([1,H,W] or [H,W]; None = ones, as the reference's loader falls back to);
-        for steps that keep mask_bufs, one plane per slot or None when built without a mask"""
+        """the alpha mask of target slot `slot` ([1,H,W] or [H,W]; None = ones, as the reference's loader falls back to)"""
         if self.mask_bufs[slot] is None:
             if mask is not None:
                 raise ValueError("this step was built without a mask (mask=False)")
@@ -126,30 +219,16 @@ class GraphedBase:
 
     def _set_exposure(self, exposure):
         """this step's [3,4] (or larger: its top 3x4 block) exposure; None = identity, as the renderers do for an image
-        without one; for steps that keep `exposure` (a device [3,4], or None when built without) and `_identity`"""
+        without one"""
         if self.exposure is not None:
             self.exposure.copy_(self._identity if exposure is None else exposure.detach()[:3, :4], non_blocking=True)
         elif exposure is not None:
             raise ValueError("this step was built without an exposure (exposure=False)")
 
-    def _raster_args(self, tanfovx, tanfovy, do_depth=0):
-        """h3dgs_raster_args of the whole frame on one GPU, flat: P rows of the scene's arrays, capacity mode"""
-        sc = self.scene
-        a = _lib.RasterArgs()
-        a.P, a.sh_degree, a.sh_coeffs = self.P, self.sh_degree, int(sc.shs.shape[1])
-        a.image_width, a.image_height = self.W, self.H
-        a.tanfovx, a.tanfovy, a.scale_modifier = float(tanfovx), float(tanfovy), 1.0
-        a.prefiltered, a.debug, a.do_depth = 0, 0, int(do_depth)
-        a.bg, a.viewmatrix, a.projmatrix, a.campos = _ptr(self.bg), _ptr(self.view), _ptr(self.proj), _ptr(self.campos)
-        a.means3D, a.shs, a.colors_precomp, a.opacities = _ptr(sc.means3D), _ptr(sc.shs), None, _ptr(sc.opacities)
-        a.scales, a.rotations, a.cov3D_precomp = _ptr(sc.scales), _ptr(sc.rotations), None
-        a.shard_count, a.shard_index = 1, 0
-        a.bin_capacity, a.sort_capacity = self.bin_capacity, self.sort_capacity
-        return a
-
-    def _fill_slot(self, slot, src):
-        """what travels with a target into its slot (subclasses add the target's mask, depth maps, ...)"""
+    def _fill_slot(self, slot, src, mask=None):
+        """what travels with a target into its slot: its alpha mask (subclasses add depth maps, ...)"""
         self.gt_bufs[slot].copy_(src, non_blocking=True)
+        self._set_mask(slot, mask)
 
     def upload_target(self, src, stream, *with_target, **kw):
         """Copy the NEXT step's target (device tensor or pinned host tensor) into one of the two static target slots on
@@ -182,9 +261,12 @@ class GraphedBase:
         torch.cuda.synchronize(self.dev)
         l0 = _lib.launch_count()
         self.graph_a = torch.cuda.CUDAGraph()
-        self.graph_b = [torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()]
         with torch.cuda.graph(self.graph_a):
             self._part_a()
+        if self._part_b is None:
+            self.launches_per_step = _lib.launch_count() - l0
+            return
+        self.graph_b = [torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()]
         with torch.cuda.graph(self.graph_b[0], pool=self.graph_a.pool()):
             self._part_b(0)
         self.launches_per_step = _lib.launch_count() - l0      # library kernels inside one replay of A + B
@@ -221,7 +303,58 @@ class GraphedBase:
         return self.status_dev
 
 
-class GraphedStep(GraphedBase):
+class GraphedLodCut(GraphedBase):
+    """What the hierarchy forms add: the device LOD cut.  h3dgs_lod_cut reads the threshold from threshold_dev (set_threshold
+    changes it between replays), leaves the cut size in `count` on the device and marks the rows after the cut -1; the
+    skybox rows follow the cut; the raster arguments carry the fields of the gather and lerp fused into K1."""
+
+    def __init__(self, scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity):
+        if not scene.hier:
+            raise ValueError(f"{type(self).__name__} drives the hierarchy path (LOD cut + fused gather/lerp)")
+        self.N_nodes = scene.nodes.shape[0]
+        _check_index_sizing(self.N_nodes, scene.means3D.shape[0])
+        super().__init__(scene, W, H, sh_degree, row_capacity, bin_capacity, sort_capacity)
+        dev = self.dev
+        self.S = scene.skybox_points
+        self.bg = bg.to(dev).float().contiguous()
+        self.threshold = float(threshold)
+        self.threshold_dev = torch.full((1,), self.threshold, dtype=torch.float32, device=dev)   # read by the cut kernels
+        self.count = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.lod_scratch = torch.empty(int(self.L.h3dgs_expand_scratch_bytes(self.N_nodes)), dtype=torch.uint8, device=dev)
+        self.sky_arange = torch.arange(self.S, dtype=torch.int64, device=dev)
+
+    def _raster_args(self, tanfovx, tanfovy):
+        sc = self.scene
+        a = super()._raster_args(tanfovx, tanfovy)
+        a.interpolation_weights, a.num_node_kids = ptr(sc.interpolation_weights), ptr(sc.num_siblings)
+        a.render_indices, a.parent_indices, a.num_source = ptr(sc.render_indices), ptr(sc.parent_indices), self.N
+        return a
+
+    def _cut(self):
+        sc = self.scene
+        if self.N > self.N_nodes:
+            sc.render_indices[self.N_nodes:].fill_(-1)  # the library marks [n, N_nodes); these are the skybox slots beyond
+        _lib.check(self.L.h3dgs_lod_cut(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
+                                        self.threshold_dev.data_ptr(), self.campos.data_ptr(), sc.render_indices.data_ptr(),
+                                        sc.parent_indices.data_ptr(), sc.nodes_for_render.data_ptr(),
+                                        sc.interpolation_weights.data_ptr(), sc.num_siblings.data_ptr(),
+                                        self.count.data_ptr(), self.lod_scratch.data_ptr(), self._stream()))
+        if self.S:
+            # skybox rows follow the cut as their own parents with t = 1, kids = 1 (render_post :220-234);
+            # a cut so large that they would not fit is reported as a row overflow by status()
+            idx = (self.count.long() + self.sky_arange).clamp_(max=self.N - 1)
+            sc.render_indices.index_copy_(0, idx, sc.skybox_inds)
+            sc.parent_indices.index_copy_(0, idx, sc.skybox_inds)
+            sc.interpolation_weights.index_fill_(0, idx, 1.0)
+            sc.num_siblings.index_fill_(0, idx, 1)
+
+    def set_threshold(self, threshold):
+        """A new LOD threshold for the next step (train_post.py:66-74 draws one per step)."""
+        self.threshold = float(threshold)
+        self.threshold_dev.fill_(self.threshold)
+
+
+class GraphedStep(GraphedLodCut):
     """scene: pipeline.Scene with a hierarchy.  The camera-independent sizes (W, H, tanfov) are fixed per
     instance (launch constants inside the graphs); camera, target and LOD threshold are device-resident
     inputs that change between replays (set_camera, upload_target / step(gt=), set_threshold)."""
@@ -229,39 +362,13 @@ class GraphedStep(GraphedBase):
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None,
                  bin_capacity=1 << 22, sort_capacity=4096, world=1, rank=0, group=None, capture=True, peer=False,
                  cyclic_log2=12):
-        if not scene.hier:
-            raise ValueError("GraphedStep drives the hierarchy path (LOD cut + fused gather/lerp)")
-        self.L = _lib.lib()
-        self.scene, self.W, self.H = scene, int(W), int(H)
-        self.threshold, self.sh_degree = float(threshold), int(sh_degree)
+        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity)
         self.world, self.rank, self.group = int(world), int(rank), group
         self.peer = bool(peer) and self.world > 1
         if self.peer and (self.world & (self.world - 1) or self.world > _lib.MAX_PEERS):
             raise ValueError("peer mode needs 2, 4 or 8 ranks")
         self.cyclic_log2 = int(cyclic_log2)
-        dev = scene.means3D.device
-        self.dev = dev
-        N = scene.means3D.shape[0]                     # rows of the parameter arrays (hierarchy + skybox)
-        self.N = N
-        self.N_nodes = scene.nodes.shape[0]
-        _check_index_sizing(self.N_nodes, N)
-        self.S = scene.skybox_points
-        self.P = int(row_capacity) if row_capacity else N
-        if not (0 < self.P <= N):
-            raise ValueError(f"row_capacity must be in (0, {N}]")
-        self.bin_capacity, self.sort_capacity = int(bin_capacity), int(sort_capacity)
-        f = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
-        # static inputs
-        self.view, self.proj, self.campos = f(16), f(16), f(3)
-        self.bg = bg.to(dev).float().contiguous()
-        # two target buffers: the upload of the next step's target (25 MB over PCIe, ~1 ms) then overlaps the WHOLE current
-        # step instead of only its graph A; graph B is captured once per buffer.  self.gt is buffer 0 (gs.gt.copy_ / step(gt=))
-        self.gt_bufs = [f(3, H, W), f(3, H, W)]
-        self.gt = self.gt_bufs[0]
-        self.threshold_dev = torch.full((1,), self.threshold, dtype=torch.float32, device=dev)   # read by the cut kernels
-        # static outputs
-        self.count = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.radii = torch.zeros(self.P, dtype=torch.int32, device=dev)
+        dev, H, W, f = self.dev, self.H, self.W, self._zeros
         self.arena = None
         if self.peer:
             from .peer import PeerArena
@@ -278,30 +385,17 @@ class GraphedStep(GraphedBase):
             self.rows = rows
         else:
             self.image = f(3, H, W)
-        self.dcolor = f(3, H, W)
         if not self.peer:
             self.loss_sum = torch.zeros(1, dtype=torch.float64, device=dev)
         self.status_dev = torch.zeros(6, dtype=torch.float64, device=dev)
-        M = scene.shs.shape[1]
-        self.grads = dict(means3D=f(N, 3), shs=f(N, M, 3), opacities=f(N, 1), scales=f(N, 3), rotations=f(N, 4))
-        self.d_means2D = f(self.P, 3)
-        chunk = (self.P + world - 1) // world
-        if self.peer:
-            self.accum = torch.zeros(max(self.P, 1) * 10, dtype=torch.float32, device=dev)      # local; partial rows travel through "stage"
-        else:
-            self.accum = torch.zeros(max(world * chunk, 1) * 10, dtype=torch.float32, device=dev)
-        self.lod_scratch = torch.empty(int(self.L.h3dgs_expand_scratch_bytes(self.N_nodes)), dtype=torch.uint8, device=dev)
-        self.sky_arange = torch.arange(self.S, dtype=torch.int64, device=dev)
-        self._init_replay()
-        self.args = self._make_args(tanfovx, tanfovy)
+        # peer: local, the partial rows travel through "stage"; NCCL: whole row blocks of the reduce-scatter
+        self._init_grads(self.P if self.peer else world * ((self.P + world - 1) // world))
+        self.args = self._raster_args(tanfovx, tanfovy)
         if capture:
             self.capture()
 
-    def _make_args(self, tanfovx, tanfovy):
-        sc = self.scene
-        a = self._raster_args(tanfovx, tanfovy)
-        a.interpolation_weights, a.num_node_kids = _ptr(sc.interpolation_weights), _ptr(sc.num_siblings)
-        a.render_indices, a.parent_indices, a.num_source = _ptr(sc.render_indices), _ptr(sc.parent_indices), self.N
+    def _raster_args(self, tanfovx, tanfovy):
+        a = super()._raster_args(tanfovx, tanfovy)
         a.shard_count, a.shard_index = self.world, self.rank
         a.grad_row_begin, a.grad_row_end = hdist.row_block(self.P, self.world, self.rank) if (self.world > 1 and not self.peer) else (0, 0)
         if self.peer:
@@ -315,30 +409,12 @@ class GraphedStep(GraphedBase):
     # ---- the two halves of the step (eager or under capture) ------------------------------
     def _part_a(self):
         """LOD cut -> forward (-> image all-gather)."""
-        sc, L = self.scene, self.L
         if self.peer:
             # every rank has finished its previous step: it no longer reads its staging area (our phase 1 stores into it) or
             # its image buffer (our forward stores into it), and its loss sum is zero again
             self.arena.barrier()
-        if self.N > self.N_nodes:
-            sc.render_indices[self.N_nodes:].fill_(-1)  # the library marks [n, N_nodes); these are the skybox slots beyond
-        _lib.check(L.h3dgs_lod_cut(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
-                                   self.threshold_dev.data_ptr(), self.campos.data_ptr(), sc.render_indices.data_ptr(), sc.parent_indices.data_ptr(),
-                                   sc.nodes_for_render.data_ptr(), sc.interpolation_weights.data_ptr(),
-                                   sc.num_siblings.data_ptr(), self.count.data_ptr(), self.lod_scratch.data_ptr(),
-                                   self._stream()))
-        if self.S:
-            # skybox rows follow the cut as their own parents with t = 1, kids = 1 (render_post :220-234);
-            # a cut so large that they would not fit is reported as a row overflow by status()
-            idx = (self.count.long() + self.sky_arange).clamp_(max=self.N - 1)
-            sc.render_indices.index_copy_(0, idx, sc.skybox_inds)
-            sc.parent_indices.index_copy_(0, idx, sc.skybox_inds)
-            sc.interpolation_weights.index_fill_(0, idx, 1.0)
-            sc.num_siblings.index_fill_(0, idx, 1)
-        out = None if self.peer else (self.slab if self.world > 1 else self.image)
-        n = C.c_int64(0)
-        _lib.check(L.h3dgs_rasterize_forward(C.byref(self.args), self._alloc_cb, None, _ptr(out),
-                                             self.radii.data_ptr(), None, C.byref(n), self._stream()))
+        self._cut()
+        self._forward(None if self.peer else (self.slab if self.world > 1 else self.image))
         if self.world > 1 and not self.peer:
             dist.all_gather_into_tensor(self.slabs, self.slab, group=self.group)
             self.image = hdist.unpack(self.slabs.view(self.world, self.rpr, 3, 16, self.W), self.H, self.W, self.world)
@@ -358,36 +434,26 @@ class GraphedStep(GraphedBase):
         else:
             _lib.check(L.h3dgs_l1_loss_grad(3, self.H, self.W, self.image.data_ptr(), gt.data_ptr(), 1.0 / numel, 1, 0,
                                             self.dcolor.data_ptr(), self.loss_sum.data_ptr(), self._stream()))
-        g = self.grads
-        outs = (g["means3D"].data_ptr(), self.d_means2D.data_ptr(), g["shs"].data_ptr(), None, g["opacities"].data_ptr(),
-                g["scales"].data_ptr(), g["rotations"].data_ptr(), None)
-        state = (self.radii.data_ptr(), self._bufs[0].data_ptr(), self._bufs[1].data_ptr(), self._bufs[2].data_ptr(),
-                 self.bin_capacity, self.dcolor.data_ptr(), None)
         if self.world == 1:
-            _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 3, self._stream()))
+            self._backward(3)
         elif self.peer:
             # phase 1 fills this rank's partial sums and pushes the rows other ranks own into their staging areas; after the
             # barrier phase 2 adds, for the rows it owns, what the ranks that touched them have staged: the whole "reduce-scatter"
             # (1 | 4: the zero-fill of the full-size gradients runs beside the replay; 2 | 8: ... and is not repeated)
-            _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 1 | 4, self._stream()))
+            self._backward(1 | 4)
             self.arena.barrier()
-            _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 2 | 8, self._stream()))
+            self._backward(2 | 8)
         else:
             # rows [P, world*chunk) of accum are zero since construction and never written: the blocks reduce cleanly
-            _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 1 | 4, self._stream()))
+            self._backward(1 | 4)
             hdist.reduce_accum(self.accum.view(torch.uint8), self.P, self.world, self.rank, self.group)
             # phase 2 rewrites exactly the own row block of d_means2D; the other rows stay zero since construction
-            _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 2 | 8, self._stream()))
+            self._backward(2 | 8)
         # status words (loss, rows needed, D, longest list, overflow flags) by one device thread; peer mode: the loss sum is
         # complete since the mid-backward barrier and is reset here for the next step (ordered before anybody's next L1
         # kernel by the start barrier)
         _lib.check(L.h3dgs_step_status(self.loss_sum.data_ptr(), 1.0 / numel, self.count.data_ptr(), self.S, self.P,
                                        self.scan_info().data_ptr(), 1 if self.peer else 0, self.status_dev.data_ptr(), self._stream()))
-
-    def set_threshold(self, threshold):
-        """A new LOD threshold for the next step (train_post.py:66-74 draws one per step)."""
-        self.threshold = float(threshold)
-        self.threshold_dev.fill_(self.threshold)
 
     def status(self):
         """One 48-byte read-back: loss, rows needed, D, longest tile list, overflow flags."""

@@ -13,10 +13,7 @@ also has them to the trained exposure and the inverse depth.  No CPU fallback.
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
+from ._lib import ptr
 
 
 def _coefficients(g_loss, g_l1, g_ssim, lam, n):
@@ -103,52 +100,6 @@ def mask_plane(mask, H, W, device):
     return mask.detach().reshape(H, W).to(device=device, dtype=torch.float32).contiguous()
 
 
-class _PostLoss(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, image, gt, lambda_dssim, exposure, mask):
-        if not image.is_cuda:
-            raise RuntimeError("post_loss needs CUDA tensors (there is no CPU fallback)")
-        img = image.detach().float().contiguous()
-        ref = gt.detach().float().contiguous()
-        if img.dim() == 4 and img.shape[0] == 1:
-            img, ref = img[0], ref[0]
-        if img.dim() != 3 or img.shape[0] != 3 or img.shape != ref.shape:
-            raise RuntimeError("expected image and gt of identical shape [3,H,W]")
-        _, H, W = img.shape
-        E = exposure_block(exposure, img.device)
-        M = mask_plane(mask, H, W, img.device)
-        sums = torch.empty(2, dtype=torch.float64, device=img.device)
-        maps = torch.empty((3, 3, H, W), dtype=torch.float32, device=img.device)
-        with torch.cuda.device(img.device):
-            _lib.check(_lib.lib().h3dgs_post_loss_forward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(E), _ptr(M),
-                                                         sums.data_ptr(), maps.data_ptr(),
-                                                         torch.cuda.current_stream().cuda_stream))
-        n = float(img.numel())
-        l1 = sums[0] / n
-        ssim = sums[1] / n
-        ctx.save_for_backward(img, ref, maps)
-        ctx.E, ctx.M = E, M
-        ctx.lam, ctx.n, ctx.in_shape = float(lambda_dssim), n, image.shape
-        loss = (1.0 - ctx.lam) * l1 + ctx.lam * (1.0 - ssim)
-        return loss.float(), l1.float(), ssim.float()
-
-    @staticmethod
-    def backward(ctx, g_loss, g_l1, g_ssim):
-        img, ref, maps = ctx.saved_tensors
-        _, H, W = img.shape
-        z = torch.zeros((), device=img.device)
-        g_loss = z if g_loss is None else g_loss
-        g_l1 = z if g_l1 is None else g_l1
-        g_ssim = z if g_ssim is None else g_ssim
-        coeffs = _coefficients(g_loss, g_l1, g_ssim, ctx.lam, ctx.n)
-        grad = torch.empty_like(img)
-        with torch.cuda.device(img.device):
-            _lib.check(_lib.lib().h3dgs_post_loss_backward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(ctx.E), _ptr(ctx.M),
-                                                          maps.data_ptr(), coeffs.data_ptr(), grad.data_ptr(),
-                                                          torch.cuda.current_stream().cuda_stream))
-        return grad.view(ctx.in_shape), None, None, None, None
-
-
 def post_loss(image, gt, lambda_dssim=0.2, exposure=None, mask=None):
     """train_post's objective on the raw rasterizer output `image` [3,H,W] -> (loss, l1, ssim) scalars:
 
@@ -157,9 +108,13 @@ def post_loss(image, gt, lambda_dssim=0.2, exposure=None, mask=None):
 
     `gt` is the target as the loader leaves it (clamped and masked already; it is used as it is).  exposure: [3,4] or
     larger (its top 3x4 block) or None (identity: render_post without an entry for the image); mask: [1,H,W] or [H,W] or
-    None (all ones).  One CUDA kernel forward and one backward; gradient to `image` only (pretrained exposures are
-    frozen, the mask is data)."""
-    return _PostLoss.apply(image, gt, lambda_dssim, exposure, mask)
+    None (all ones).  One CUDA kernel forward and one backward (single_loss's, without the depth term); gradient to
+    `image` only (pretrained exposures are frozen, the mask is data)."""
+    if image.dim() == 4 and image.shape[0] == 1:
+        image, gt = image[0], gt[0]
+    exposure = None if exposure is None else exposure.detach()
+    loss, _, l1, ssim, _ = _SingleLoss.apply(image, None, exposure, gt, lambda_dssim, mask, None, None, 0.0)
+    return loss, l1, ssim
 
 
 class _SingleLoss(torch.autograd.Function):
@@ -167,7 +122,7 @@ class _SingleLoss(torch.autograd.Function):
     def forward(ctx, image, invdepth, exposure, gt, lambda_dssim, mask, mono_invdepth, depth_mask, depth_weight):
         from diff_gaussian_rasterization._C import _on_device
         if not _on_device(image):
-            raise RuntimeError("single_loss needs CUDA tensors (there is no CPU fallback)")
+            raise RuntimeError("post_loss / single_loss need CUDA tensors (there is no CPU fallback)")
         img = image.detach().float().contiguous()
         ref = gt.detach().float().contiguous()
         if img.dim() != 3 or img.shape[0] != 3 or img.shape != ref.shape:
@@ -182,7 +137,7 @@ class _SingleLoss(torch.autograd.Function):
         st = torch.cuda.current_stream(dev).cuda_stream
         depth = mono_invdepth is not None
         with torch.cuda.device(dev):
-            _lib.check(L.h3dgs_post_loss_forward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(E), _ptr(M), sums.data_ptr(),
+            _lib.check(L.h3dgs_post_loss_forward(H, W, img.data_ptr(), ref.data_ptr(), ptr(E), ptr(M), sums.data_ptr(),
                                                  maps.data_ptr(), st))
             if depth:
                 if invdepth is None or invdepth.numel() != H * W:
@@ -227,13 +182,13 @@ class _SingleLoss(torch.autograd.Function):
         with torch.cuda.device(dev):
             if ctx.exposure_like is not None:
                 dE = torch.empty((3, 4), dtype=torch.float64, device=dev)
-                _lib.check(L.h3dgs_post_loss_backward_exposure(H, W, img.data_ptr(), ref.data_ptr(), _ptr(ctx.E), _ptr(ctx.M),
+                _lib.check(L.h3dgs_post_loss_backward_exposure(H, W, img.data_ptr(), ref.data_ptr(), ptr(ctx.E), ptr(ctx.M),
                                                                maps.data_ptr(), coeffs.data_ptr(), grad.data_ptr(),
                                                                dE.data_ptr(), st))
                 g_E = torch.zeros_like(ctx.exposure_like)
                 g_E[:3, :4] = dE.to(g_E.dtype)
             else:
-                _lib.check(L.h3dgs_post_loss_backward(H, W, img.data_ptr(), ref.data_ptr(), _ptr(ctx.E), _ptr(ctx.M),
+                _lib.check(L.h3dgs_post_loss_backward(H, W, img.data_ptr(), ref.data_ptr(), ptr(ctx.E), ptr(ctx.M),
                                                       maps.data_ptr(), coeffs.data_ptr(), grad.data_ptr(), st))
             if ctx.dinv is not None and ctx.needs_input_grad[1]:
                 # the forward's one pass wrote the gradient with the term's sum; times 1 under loss.backward(): exact

@@ -18,13 +18,10 @@ GraphedStep; the caller re-runs it through pipeline.post_step, the exact path wi
 respect to the activated Scene tensors; the optimizer and the skybox / anchor gradient zeroing of train_post.py:167-181
 stay the caller's.  One GPU only: the SSIM window reaches across the tile-row shards of the sharded forms.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
-from .graphstep import GraphedStep, _ptr
-from .loss import _coefficients
+from .graphstep import GraphedStep
 
 
 class GraphedPostStep(GraphedStep):
@@ -41,45 +38,18 @@ class GraphedPostStep(GraphedStep):
             raise ValueError("GraphedPostStep runs on one GPU: the SSIM window reaches across the tile-row shards")
         super().__init__(scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=sh_degree, row_capacity=row_capacity,
                          bin_capacity=bin_capacity, sort_capacity=sort_capacity, capture=False)
-        dev, H, W = self.dev, self.H, self.W
-        self.lambda_dssim = float(lambda_dssim)
-        self._identity = torch.eye(3, 4, device=dev)
-        self.exposure = self._identity.clone() if exposure else None
-        # one mask per target slot: a mask travels with its target
-        self.mask_bufs = [torch.ones((H, W), device=dev), torch.ones((H, W), device=dev)] if mask else [None, None]
-        self.mask = self.mask_bufs[0]
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
-        self.maps = torch.zeros((3, 3, H, W), dtype=torch.float32, device=dev)
-        self.status_dev = torch.zeros(8, dtype=torch.float64, device=dev)
-        # the weights of sign(a - gt) and of the SSIM-sum gradient for loss.backward(), formed as post_loss's backward
-        # forms them, so that the graphed dL/dimage equals the eager one bit for bit
-        one, zero = torch.ones((), device=dev), torch.zeros((), device=dev)
-        self.coeffs = _coefficients(one, zero, zero, self.lambda_dssim, float(3 * H * W))
+        self._init_post_loss(lambda_dssim, exposure, mask)
+        self.status_dev = torch.zeros(8, dtype=torch.float64, device=self.dev)
         if capture:
             self.capture()
 
     def _part_b(self, slot=0):
         """The objective against target slot `slot` and its mask, its gradient, the backward, the status words."""
-        L, st = self.L, self._stream()
-        gt, M = self.gt_bufs[slot], self.mask_bufs[slot]
-        _lib.check(L.h3dgs_post_loss_forward(self.H, self.W, self.image.data_ptr(), gt.data_ptr(), _ptr(self.exposure),
-                                             _ptr(M), self.sums.data_ptr(), self.maps.data_ptr(), st))
-        _lib.check(L.h3dgs_post_loss_backward(self.H, self.W, self.image.data_ptr(), gt.data_ptr(), _ptr(self.exposure),
-                                              _ptr(M), self.maps.data_ptr(), self.coeffs.data_ptr(), self.dcolor.data_ptr(), st))
-        g = self.grads
-        outs = (g["means3D"].data_ptr(), self.d_means2D.data_ptr(), g["shs"].data_ptr(), None, g["opacities"].data_ptr(),
-                g["scales"].data_ptr(), g["rotations"].data_ptr(), None)
-        state = (self.radii.data_ptr(), self._bufs[0].data_ptr(), self._bufs[1].data_ptr(), self._bufs[2].data_ptr(),
-                 self.bin_capacity, self.dcolor.data_ptr(), None)
-        _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 3, st))
-        _lib.check(L.h3dgs_post_step_status(self.sums.data_ptr(), 1.0 / self.image.numel(), self.lambda_dssim,
-                                            self.count.data_ptr(), self.S, self.P, self.scan_info().data_ptr(),
-                                            self.status_dev.data_ptr(), st))
-
-    def _fill_slot(self, slot, src, mask=None):
-        """upload_target(src, stream, mask): the NEXT step's target and its alpha mask ([1,H,W] or [H,W]; None = ones)"""
-        self.gt_bufs[slot].copy_(src, non_blocking=True)
-        self._set_mask(slot, mask)
+        self._post_loss(slot)
+        self._backward(3)
+        _lib.check(self.L.h3dgs_post_step_status(self.sums.data_ptr(), 1.0 / self.image.numel(), self.lambda_dssim,
+                                                 self.count.data_ptr(), self.S, self.P, self.scan_info().data_ptr(),
+                                                 self.status_dev.data_ptr(), self._stream()))
 
     def step(self, cam=None, gt=None, mask=None, exposure=None, gt_ready=None):
         """cam, gt (+ its mask; None = ones): optional new inputs, copied into the static buffers (the target into slot

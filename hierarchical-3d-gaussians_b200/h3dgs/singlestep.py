@@ -23,13 +23,11 @@ exact path with the same kernels.  Gradients are with respect to the activated S
 Adam over the rows with a gradient, the exposure's Adam), densify_and_prune, reset_opacity and the big-Gaussian
 rescale of train_single.py:150-186 stay the caller's.  One GPU only: the SSIM window reaches across tile-row shards.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
-from .graphstep import GraphedBase, _ptr
-from .loss import _coefficients
+from ._lib import ptr
+from .graphstep import GraphedBase
 from .pipeline import DensifyStats
 
 
@@ -58,51 +56,27 @@ class GraphedSingleStep(GraphedBase):
             raise ValueError("GraphedSingleStep runs on one GPU: the SSIM window reaches across the tile-row shards")
         if scene.hier:
             raise ValueError("GraphedSingleStep trains a flat scene (train_single.py); a hierarchy goes through GraphedPostStep")
-        self.L = _lib.lib()
-        self.scene, self.W, self.H = scene, int(W), int(H)
-        self.sh_degree, self.lambda_dssim = int(sh_degree), float(lambda_dssim)
-        dev = self.dev = scene.means3D.device
-        N = self.N = self.P = scene.means3D.shape[0]
-        self.bin_capacity, self.sort_capacity = int(bin_capacity), int(sort_capacity)
-        H, W = self.H, self.W
-        f = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
-        # inputs that change between replays
-        self.view, self.proj, self.campos, self.bg = f(16), f(16), f(3), f(3)
-        self._identity = torch.eye(3, 4, device=dev)
-        self.exposure = self._identity.clone() if exposure else None
-        self.depth_weight = f(1)
-        self.gt_bufs = [f(3, H, W), f(3, H, W)]
-        self.gt = self.gt_bufs[0]
-        # what travels with a target, one per slot
-        self.mask_bufs = [torch.ones((H, W), device=dev), torch.ones((H, W), device=dev)] if mask else [None, None]
+        super().__init__(scene, W, H, sh_degree, None, bin_capacity, sort_capacity)
+        dev, H, W, N, f = self.dev, self.H, self.W, self.N, self._zeros
+        # inputs that change between replays, and what travels with a target, one per slot
+        self.bg, self.depth_weight = f(3), f(1)
+        self._init_post_loss(lambda_dssim, exposure, mask)
         self.mono_bufs = [f(H, W), f(H, W)] if depth else [None, None]
         self.depth_mask_bufs = [f(H, W), f(H, W)] if depth else [None, None]
         # outputs
         self.image, self.invdepth = f(3, H, W), f(1, H, W)
-        self.radii = torch.zeros(N, dtype=torch.int32, device=dev)
-        self.dcolor = f(3, H, W)
         self.dinvdepth = f(H, W) if depth else None
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
         self.depth_sum = torch.zeros(1, dtype=torch.float64, device=dev) if depth else None
-        self.maps = f(3, 3, H, W)
         self.exposure_grad64 = torch.zeros((3, 4), dtype=torch.float64, device=dev) if exposure else None
         self.exposure_grad = f(3, 4) if exposure else None
         self.status_dev = torch.zeros(8, dtype=torch.float64, device=dev)
-        M = scene.shs.shape[1]
-        self.grads = dict(means3D=f(N, 3), shs=f(N, M, 3), opacities=f(N, 1), scales=f(N, 3), rotations=f(N, 4))
-        self.d_means2D = f(N, 3)
-        self.accum = torch.zeros(max(N, 1) * 10, dtype=torch.float32, device=dev)
+        self._init_grads(N)
         if isinstance(stats, DensifyStats):
             if stats.denom.shape[0] != N:
                 raise ValueError(f"the statistics hold {stats.denom.shape[0]} rows, the scene {N}")
             self.stats = stats
         else:
             self.stats = DensifyStats(N, dev) if stats else None
-        # the weights of sign(a - gt) and of the SSIM-sum gradient for loss.backward(), formed as single_loss's backward
-        # forms them, so that the graphed dL/dimage equals the eager one bit for bit
-        one, zero = torch.ones((), device=dev), torch.zeros((), device=dev)
-        self.coeffs = _coefficients(one, zero, zero, self.lambda_dssim, float(3 * H * W))
-        self._init_replay()
         self._count_stats = True
         self.args = self._raster_args(tanfovx, tanfovy, do_depth=1)
         if capture:
@@ -120,40 +94,25 @@ class GraphedSingleStep(GraphedBase):
     # ---- the two halves of the step (eager or under capture) ------------------------------
     def _part_a(self):
         """capacity-mode forward of all N rows, with the inverse depth"""
-        n = C.c_int64(0)
-        _lib.check(self.L.h3dgs_rasterize_forward(C.byref(self.args), self._alloc_cb, None, self.image.data_ptr(),
-                                                  self.radii.data_ptr(), self.invdepth.data_ptr(), C.byref(n), self._stream()))
+        self._forward(self.image, self.invdepth)
 
     def _part_b(self, slot=0):
         """The objective against slot `slot`, its gradients, the backward, the statistics, the status words."""
         L, st, H, W = self.L, self._stream(), self.H, self.W
-        gt, M = self.gt_bufs[slot], self.mask_bufs[slot]
-        loss_args = (H, W, self.image.data_ptr(), gt.data_ptr(), _ptr(self.exposure), _ptr(M))
-        _lib.check(L.h3dgs_post_loss_forward(*loss_args, self.sums.data_ptr(), self.maps.data_ptr(), st))
-        if self.exposure is not None:
-            _lib.check(L.h3dgs_post_loss_backward_exposure(*loss_args, self.maps.data_ptr(), self.coeffs.data_ptr(),
-                                                           self.dcolor.data_ptr(), self.exposure_grad64.data_ptr(), st))
-        else:
-            _lib.check(L.h3dgs_post_loss_backward(*loss_args, self.maps.data_ptr(), self.coeffs.data_ptr(),
-                                                  self.dcolor.data_ptr(), st))
+        self._post_loss(slot, self.exposure_grad64)
         if self.dinvdepth is not None:
             _lib.check(L.h3dgs_invdepth_l1_grad(H, W, self.invdepth.data_ptr(), self.mono_bufs[slot].data_ptr(),
                                                 self.depth_mask_bufs[slot].data_ptr(), self.depth_weight.data_ptr(),
                                                 self.dinvdepth.data_ptr(), self.depth_sum.data_ptr(), st))
-        g = self.grads
-        outs = (g["means3D"].data_ptr(), self.d_means2D.data_ptr(), g["shs"].data_ptr(), None, g["opacities"].data_ptr(),
-                g["scales"].data_ptr(), g["rotations"].data_ptr(), None)
-        state = (self.radii.data_ptr(), self._bufs[0].data_ptr(), self._bufs[1].data_ptr(), self._bufs[2].data_ptr(),
-                 self.bin_capacity, self.dcolor.data_ptr(), _ptr(self.dinvdepth))
-        _lib.check(L.h3dgs_rasterize_backward(C.byref(self.args), *state, *outs, self.accum.data_ptr(), 3, st))
+        self._backward(3)
         info = self.scan_info().data_ptr()
         if self.stats is not None and self._count_stats:
             s = self.stats
             _lib.check(L.h3dgs_densify_stats(self.P, self.radii.data_ptr(), self.d_means2D.data_ptr(), s.max_radii2D.data_ptr(),
                                              s.xyz_gradient_accum.data_ptr(), s.denom.data_ptr(), info, st))
-        _lib.check(L.h3dgs_single_step_status(self.sums.data_ptr(), _ptr(self.depth_sum), self.depth_weight.data_ptr(),
+        _lib.check(L.h3dgs_single_step_status(self.sums.data_ptr(), ptr(self.depth_sum), self.depth_weight.data_ptr(),
                                               1.0 / (3 * H * W), 1.0 / (H * W), self.lambda_dssim, info,
-                                              _ptr(self.exposure_grad64), _ptr(self.exposure_grad), self.status_dev.data_ptr(), st))
+                                              ptr(self.exposure_grad64), ptr(self.exposure_grad), self.status_dev.data_ptr(), st))
 
     # ---- driving --------------------------------------------------------------------------
     def set_background(self, bg):

@@ -193,6 +193,35 @@ def test_overflowed_frames_are_rerun_and_equal_an_ample_capacity():
         assert np.array_equal(small["rows"][..., 3], rows)
 
 
+def test_a_camera_without_a_mask_is_evaluated_with_ones():
+    """a None entry in masks: ones for that camera (the reference loader's fallback), in the replayed frames (not the mask
+    of the camera before it) and in the frames re-run through the exact path"""
+    import torch
+    from h3dgs import pipeline
+    from h3dgs.evaluate import evaluate_hierarchy
+    cam, h = _scene(skybox=50)
+    scene = pipeline.Scene(h, requires_grad=False)
+    bg = torch.zeros(3, device="cuda")
+    dcams = [pipeline.DeviceCamera(c) for c in _cams(cam.W, cam.H)]
+    targets = _targets(scene, dcams, bg)
+    rng = np.random.default_rng(8)
+    masks = [torch.tensor((rng.uniform(size=(1, cam.H, cam.W)) > 0.2).astype(np.float32), device="cuda") for _ in dcams]
+    masks[1] = None
+    with torch.no_grad():
+        n = pipeline.render_hier_fused(scene, dcams[1], bg, pipeline.fov_threshold(0.0, dcams[1]))[2]
+    # one row short of camera 1's finest cut: that frame is re-run exactly, its coarser ones are replayed
+    caps = dict(row_capacity=n + 50 - 1, bin_capacity=1 << 21, sort_capacity=8192)
+    res = evaluate_hierarchy(scene, dcams, targets, TAUS, masks=masks, capacities=caps)
+    rerun_1 = [ti for ti, ci, _ in res["flagged"] if ci == 1]
+    assert 0 in rerun_1 and len(rerun_1) < len(TAUS)
+    ones = [torch.ones((1, cam.H, cam.W), device="cuda") if m is None else m for m in masks]
+    ref = _reference_loop(scene, dcams, targets, TAUS, ones, None, False, bg)
+    for tau in TAUS:
+        p, s, _ = ref[tau]
+        assert abs(res["psnr"][tau] - p) <= 1e-4, (tau, res["psnr"][tau], p)
+        assert abs(res["ssim"][tau] - s) <= 1e-5 * abs(s), (tau, res["ssim"][tau], s)
+
+
 def test_the_sweep_never_synchronises_the_host():
     import torch
     from h3dgs import pipeline
