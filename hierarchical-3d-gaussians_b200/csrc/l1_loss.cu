@@ -133,6 +133,7 @@ densify_stats_kernel(int P, const int* __restrict__ radii, const float* __restri
     if (r <= 0) return;
     const float rf = (float)r, mr = max_radii2D[i];
     max_radii2D[i] = (mr != mr || mr > rf) ? mr : rf;
+    if (!denom) return;                                     // max_radii2D only (train_coarse.py:125)
     const float x = dL_dmeans2D[3 * (size_t)i], y = dL_dmeans2D[3 * (size_t)i + 1];
     const float n = sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))), a = xyz_gradient_accum[i];
     xyz_gradient_accum[i] = (n != n || n > a) ? n : a;
@@ -162,7 +163,7 @@ extern "C" int h3dgs_invdepth_l1_grad(int32_t H, int32_t W, const float* invdept
 extern "C" int h3dgs_densify_stats(int32_t P, const int32_t* radii, const float* dL_dmeans2D, float* max_radii2D,
                                    float* xyz_gradient_accum, float* denom, const uint32_t* scan_info, void* stream)
 {
-    if (P < 0 || (P > 0 && (!radii || !dL_dmeans2D || !max_radii2D || !xyz_gradient_accum || !denom))) { set_error("densify_stats: bad arguments"); return H3DGS_EINVAL; }
+    if (P < 0 || (P > 0 && (!radii || !max_radii2D || !xyz_gradient_accum != !denom || (denom && !dL_dmeans2D)))) { set_error("densify_stats: bad arguments"); return H3DGS_EINVAL; }
     if (P == 0) return H3DGS_OK;
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope prof(H3DGS_STAGE_DENSIFY_STATS, s);

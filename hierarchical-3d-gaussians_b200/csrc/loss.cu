@@ -45,7 +45,8 @@ __device__ __forceinline__ float exposed(const float* __restrict__ img, size_t p
 
 // kPost = false: the loss of img against gt (h3dgs_l1_ssim_forward).  kPost = true: the loss of a = clamp(y, 0, 1) * mask
 // against gt as it is, y = exposed(img) or img[c] (h3dgs_post_loss_forward; C = 3); exposure and mask may be NULL.
-template <bool kPost>
+// kClamp = false (train_coarse's objective, h3dgs_coarse_loss_forward): a = y * mask, unclamped.
+template <bool kPost, bool kClamp = true>
 __global__ void __launch_bounds__(256)
 l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
                        double* __restrict__ sums, float* __restrict__ maps, size_t map_stride, const LossWindow win,
@@ -68,7 +69,7 @@ l1_ssim_forward_kernel(int H, int W, const float* __restrict__ img, const float*
             if (in) {
                 const size_t p = (size_t)gy * W + gx;
                 const float y = exposure ? exposed(img, plane, p, exposure, c) : ia[p];
-                a = fminf(fmaxf(y, 0.f), 1.f);
+                a = kClamp ? fminf(fmaxf(y, 0.f), 1.f) : y;
                 if (mask) a *= mask[p];
                 b = ib[p];                                      // the loader clamped and masked the target already
             }
@@ -188,7 +189,9 @@ l1_ssim_backward_kernel(int H, int W, const float* __restrict__ img, const float
 // twelve per-pixel terms img_k * g_c (k, c < 3; one rounded product each) and g_c are summed over the CTA in fp32 (xor
 // butterfly over the warp, offsets 16 .. 1), the eight warp sums are added in fp64 in warp order and one fp64 atomic
 // per CTA and entry adds them to dL_dE.  dL/dimg does not depend on the flag.
-template <bool kGradE>
+// kClamp = false (train_coarse, h3dgs_coarse_loss_backward): a = y * m and dL/dy_c = m * (...) without the clamp
+// indicator -- the rasterizer clamps colours only below, so y > 1 occurs and its gradient passes.
+template <bool kGradE, bool kClamp = true>
 __global__ void __launch_bounds__(256)
 post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
                           const float* __restrict__ exposure, const float* __restrict__ mask,
@@ -215,13 +218,13 @@ post_loss_backward_kernel(int H, int W, const float* __restrict__ img, const flo
         g[c] = 0.f;
         if (own) {
             const float y = exposure ? exposed(img, plane, p, exposure, c) : img[(size_t)c * plane + p];
-            float a = fminf(fmaxf(y, 0.f), 1.f);
+            float a = kClamp ? fminf(fmaxf(y, 0.f), 1.f) : y;
             if (mask) a *= m;
             const float b = gt[(size_t)c * plane + p];
             const float sgn = (a > b) ? 1.f : ((a < b) ? -1.f : 0.f);
             float d = k0 * sgn + k1 * (c0 + 2.f * a * c1 + b * c2);
             if (mask) d = __fmul_rn(m, d);
-            g[c] = (y >= 0.f && y <= 1.f) ? d : 0.f;
+            g[c] = (!kClamp || (y >= 0.f && y <= 1.f)) ? d : 0.f;
         }
     }
     if (kGradE) {
@@ -366,6 +369,50 @@ extern "C" int h3dgs_post_loss_backward_exposure(int32_t H, int32_t W, const flo
     ProfScope prof(H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, s);
     post_loss_backward_kernel<true><<<grid, 256, 0, s>>>(H, W, img, gt, exposure, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, dL_dexposure, make_loss_window());
     H3_LAUNCHED("post_loss_backward_exposure", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_coarse_loss_forward(int32_t H, int32_t W, const float* img, const float* gt, const float* mask,
+                                         double* sums, float* maps, void* stream)
+{
+    if (H <= 0 || W <= 0 || !img || !gt || !sums) { set_error("coarse_loss_forward: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    H3_CUDA(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
+    const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 3);
+    l1_ssim_forward_kernel<true, false><<<grid, 256, 0, s>>>(H, W, img, gt, sums, maps, (size_t)3 * H * W, make_loss_window(), nullptr, mask);
+    H3_LAUNCHED("coarse_loss_forward", 0, s);
+    return H3DGS_OK;
+}
+
+extern "C" int h3dgs_coarse_loss_backward(int32_t H, int32_t W, const float* img, const float* gt, const float* mask,
+                                          const float* maps, const float* coeffs, float* dL_dimg, void* stream)
+{
+    if (H <= 0 || W <= 0 || !img || !gt || !maps || !coeffs || !dL_dimg) { set_error("coarse_loss_backward: bad arguments"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    const dim3 grid((W + kTS - 1) / kTS, (H + kTS - 1) / kTS, 1);
+    post_loss_backward_kernel<false, false><<<grid, 256, 0, s>>>(H, W, img, gt, nullptr, mask, maps, (size_t)3 * H * W, coeffs, dL_dimg, nullptr, make_loss_window());
+    H3_LAUNCHED("coarse_loss_backward", 0, s);
+    return H3DGS_OK;
+}
+
+// One thread: the six status words of train_coarse's step (h3dgs/coarsestep.py) -- loss, L1, SSIM, D, longest tile list,
+// binning overflow.
+__global__ void coarse_step_status_kernel(const double* __restrict__ sums, double inv_numel, double lambda_dssim,
+                                          const uint32_t* __restrict__ scan_info, double* __restrict__ out)
+{
+    const double l1 = sums[0] * inv_numel, ssim = sums[1] * inv_numel;
+    out[0] = (1.0 - lambda_dssim) * l1 + lambda_dssim * (1.0 - ssim);
+    out[1] = l1; out[2] = ssim;
+    out[3] = (double)scan_info[0]; out[4] = (double)scan_info[1]; out[5] = (double)scan_info[2];
+}
+
+extern "C" int h3dgs_coarse_step_status(const double* sums, double inv_numel, double lambda_dssim, const uint32_t* scan_info,
+                                        double* out, void* stream)
+{
+    if (!sums || !scan_info || !out) { set_error("coarse_step_status: NULL argument"); return H3DGS_EINVAL; }
+    cudaStream_t s = (cudaStream_t)stream;
+    coarse_step_status_kernel<<<1, 1, 0, s>>>(sums, inv_numel, lambda_dssim, scan_info, out);
+    H3_LAUNCHED("coarse_step_status", 0, s);
     return H3DGS_OK;
 }
 

@@ -2,12 +2,11 @@
 // (replaces scene/OurAdam.py:249-337, driven by train_single.py:170-178 with relevant = rows whose
 // opacity gradient is non-zero).  The reference gathers the rows of param / grad / exp_avg / exp_avg_sq
 // with fancy indexing, runs ~10 elementwise kernels on the copies and scatters three tensors back, per
-// parameter group; here one kernel per parameter tensor updates the rows in place.  Same arithmetic as the
-// reference's non-capturable path (amsgrad off, weight_decay 0):
-//   m = b1 m + (1-b1) g ;  v = b2 v + (1-b2) g^2 ;  p -= step_size * m / (sqrt(v)/sqrt(bc2) + eps)
-// with step_size = lr / bc1, bc1 = 1 - b1^step, bc2 = 1 - b2^step computed by the caller (host doubles,
-// as the reference does with Python floats).  HBM-bound: 4 reads + 3 writes of 4 B per touched element.
+// parameter group; here one kernel per parameter tensor updates the rows in place, with the arithmetic of adam.cuh
+// (bc1 = 1 - b1^step, bc2 = 1 - b2^step computed by the caller in host doubles, as the reference does with Python
+// floats).  A negative entry of `relevant` is skipped; relevant == NULL is every row of [0, num_relevant).  HBM-bound: 4 reads + 3 writes of 4 B per touched element.
 #include "common.cuh"
+#include "adam.cuh"
 
 namespace h3dgs {
 
@@ -21,14 +20,12 @@ sparse_adam_kernel(int64_t R, int width, const int64_t* __restrict__ relevant, f
     if (t >= R * width) return;
     const int64_t r = t / width;
     const int c = (int)(t - r * width);
-    const size_t o = (size_t)relevant[r] * width + c;
-    const float g = grad[o];
-    // exp_avg.mul_(beta1).add_(grad, alpha=1-beta1) ; exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1-beta2)
-    const float m = __fadd_rn(__fmul_rn(exp_avg[o], beta1), __fmul_rn(one_minus_b1, g));
-    const float v = __fadd_rn(__fmul_rn(exp_avg_sq[o], beta2), __fmul_rn(one_minus_b2, __fmul_rn(g, g)));
-    // denom = (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps) ; param.addcdiv_(exp_avg, denom, value=-step_size)
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
-    param[o] = __fadd_rn(param[o], __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+    const int64_t row = relevant ? relevant[r] : r;
+    if (row < 0) return;                                    // a skipped entry (h3dgs.optim.Adam's [R,2] row sets)
+    const size_t o = (size_t)row * width + c;
+    float p = param[o], m = exp_avg[o], v = exp_avg_sq[o];
+    adam_element(p, grad[o], m, v, beta1, beta2, one_minus_b1, one_minus_b2, step_size, bc2_sqrt, eps);
+    param[o] = p;
     exp_avg[o] = m;
     exp_avg_sq[o] = v;
 }
@@ -40,7 +37,7 @@ extern "C" int h3dgs_sparse_adam(int64_t num_relevant, int32_t width, const int6
                                  double beta2, double eps, int64_t step, void* stream)
 {
     using namespace h3dgs;
-    if (num_relevant < 0 || width <= 0 || step <= 0 || (num_relevant > 0 && (!relevant || !param || !grad || !exp_avg || !exp_avg_sq))) {
+    if (num_relevant < 0 || width <= 0 || step <= 0 || (num_relevant > 0 && (!param || !grad || !exp_avg || !exp_avg_sq))) {
         set_error("sparse_adam: bad arguments"); return H3DGS_EINVAL;
     }
     if (num_relevant == 0) return H3DGS_OK;

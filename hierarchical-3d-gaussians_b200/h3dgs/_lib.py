@@ -28,6 +28,7 @@ EXPORTS = [
     "h3dgs_merge_hierarchies_scratch_bytes", "h3dgs_merge_hierarchies",
     "h3dgs_post_loss_forward", "h3dgs_post_loss_backward", "h3dgs_post_step_status",
     "h3dgs_post_loss_backward_exposure", "h3dgs_invdepth_l1_grad", "h3dgs_densify_stats", "h3dgs_single_step_status",
+    "h3dgs_coarse_loss_forward", "h3dgs_coarse_loss_backward", "h3dgs_coarse_step_status", "h3dgs_coarse_param_step",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -51,6 +52,24 @@ class RasterArgs(C.Structure):
         ("bin_capacity", C.c_int64), ("sort_capacity", C.c_int32),
         ("peer_count", C.c_int32), ("grad_cyclic_log2", C.c_int32),
         ("peer_image", C.c_void_p * 8), ("peer_stage", C.c_void_p * 8),
+    ]
+
+
+COARSE_SCRATCH_BYTES = 64     # H3DGS_COARSE_SCRATCH_BYTES
+COARSE_STEP, COARSE_ACTIVATE, COARSE_BIAS = 0, 1, 2
+
+
+class CoarseArgs(C.Structure):
+    """struct h3dgs_coarse_args"""
+    _fields_ = [
+        ("N", C.c_int32), ("sh_coeffs", C.c_int32), ("skybox_points", C.c_int32), ("rescale_threshold", C.c_float),
+        ("params", C.c_void_p * 6), ("exp_avg", C.c_void_p * 6), ("exp_avg_sq", C.c_void_p * 6),
+        ("lr", C.c_double * 6), ("beta1", C.c_double * 6), ("beta2", C.c_double * 6), ("eps", C.c_double * 6),
+        ("step", C.c_void_p), ("scratch", C.c_void_p),
+        ("grad_means3D", C.c_void_p), ("grad_shs", C.c_void_p), ("grad_opacities", C.c_void_p), ("grad_scales", C.c_void_p),
+        ("grad_rotations", C.c_void_p),
+        ("means3D", C.c_void_p), ("shs", C.c_void_p), ("opacities", C.c_void_p), ("scales", C.c_void_p),
+        ("rotations", C.c_void_p), ("scan_info", C.c_void_p),
     ]
 
 
@@ -151,6 +170,15 @@ def bind(l):
         l.h3dgs_post_loss_backward_exposure.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 9
         l.h3dgs_single_step_status.restype = C.c_int
         l.h3dgs_single_step_status.argtypes = [C.c_void_p] * 3 + [C.c_double] * 3 + [C.c_void_p] * 5
+        l.h3dgs_coarse_loss_forward.restype = C.c_int
+        l.h3dgs_coarse_loss_forward.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 6
+        l.h3dgs_coarse_loss_backward.restype = C.c_int
+        l.h3dgs_coarse_loss_backward.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
+        l.h3dgs_coarse_step_status.restype = C.c_int
+        l.h3dgs_coarse_step_status.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
+    if hasattr(l, "h3dgs_coarse_param_step"):    # train_coarse's parameter step (an emulation build has it when it compiles coarse_param.cu)
+        l.h3dgs_coarse_param_step.restype = C.c_int
+        l.h3dgs_coarse_param_step.argtypes = [C.POINTER(CoarseArgs), C.c_int32, C.c_void_p]
     l.h3dgs_invdepth_l1_grad.restype = C.c_int
     l.h3dgs_invdepth_l1_grad.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
     l.h3dgs_densify_stats.restype = C.c_int

@@ -217,3 +217,55 @@ def single_loss(image, invdepth, gt, lambda_dssim=0.2, exposure=None, mask=None,
     if mono_invdepth is not None and not torch.is_tensor(depth_weight) and float(depth_weight) == 0.0:
         mono_invdepth = None
     return _SingleLoss.apply(image, invdepth, exposure, gt, lambda_dssim, mask, mono_invdepth, depth_mask, depth_weight)
+
+
+class _CoarseLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, image, gt, lambda_dssim, mask):
+        from diff_gaussian_rasterization._C import _on_device
+        if not _on_device(image):
+            raise RuntimeError("coarse_loss needs CUDA tensors (there is no CPU fallback)")
+        img = image.detach().float().contiguous()
+        ref = gt.detach().float().contiguous()
+        if img.dim() != 3 or img.shape[0] != 3 or img.shape != ref.shape:
+            raise RuntimeError("expected image and gt of identical shape [3,H,W]")
+        _, H, W = img.shape
+        dev = img.device
+        M = mask_plane(mask, H, W, dev)
+        sums = torch.empty(2, dtype=torch.float64, device=dev)
+        maps = torch.empty((3, 3, H, W), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().h3dgs_coarse_loss_forward(H, W, img.data_ptr(), ref.data_ptr(), ptr(M), sums.data_ptr(),
+                                                           maps.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        n = float(img.numel())
+        l1, ssim = sums[0] / n, sums[1] / n
+        ctx.save_for_backward(img, ref, maps)
+        ctx.M, ctx.lam, ctx.n, ctx.in_shape = M, float(lambda_dssim), n, image.shape
+        loss = (1.0 - ctx.lam) * l1 + ctx.lam * (1.0 - ssim)
+        return loss.float(), l1.float(), ssim.float()
+
+    @staticmethod
+    def backward(ctx, g_loss, g_l1, g_ssim):
+        img, ref, maps = ctx.saved_tensors
+        _, H, W = img.shape
+        dev = img.device
+        coeffs = _coefficients(g_loss, g_l1, g_ssim, ctx.lam, ctx.n)
+        grad = torch.empty_like(img)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().h3dgs_coarse_loss_backward(H, W, img.data_ptr(), ref.data_ptr(), ptr(ctx.M), maps.data_ptr(),
+                                                            coeffs.data_ptr(), grad.data_ptr(),
+                                                            torch.cuda.current_stream(dev).cuda_stream))
+        return grad.view(ctx.in_shape), None, None, None
+
+
+def coarse_loss(image, gt, lambda_dssim=0.2, mask=None):
+    """train_coarse's objective on render_coarse's image [3,H,W] -> (loss, l1, ssim) scalars:
+
+        a    = image * mask                                         (train_coarse.py:113-116; no exposure, no clamp)
+        loss = (1-l) * mean|a - gt| + l * (1 - SSIM(a, gt))
+
+    mask: [1,H,W] or [H,W] or None (the camera has no alpha mask: a = image).  One CUDA kernel forward and one backward;
+    the gradient reaches `image` for every value, above 1 included (render_coarse's colours are clamped only below)."""
+    if image.dim() == 4 and image.shape[0] == 1:
+        image, gt = image[0], gt[0]
+    return _CoarseLoss.apply(image, gt, lambda_dssim, mask)

@@ -247,6 +247,29 @@ def single_step(scene, cam, bg, gt, lambda_dssim=0.2, exposure=None, mask=None, 
     return out, radii, means2D
 
 
+def coarse_step(state, scene, cam, bg, gt, cameras_extent, lambda_dssim=0.2, mask=None, sh_degree=0, update=True):
+    """One iteration of train_coarse's loop body (train_coarse.py:97-145) on the exact path: render_coarse (render_flat
+    of the activated rows in `scene`, state.make_scene()), the objective (h3dgs.loss.coarse_loss: alpha mask, (1-l) L1
+    + l (1 - SSIM), no clamp), backward, max_radii2D, then with update=True the parameter step of
+    h3dgs.coarsestep.CoarseState (skybox lock, relevance, Adam, rescale) on the gradients that landed in the scene's
+    tensors, which also refreshes the activated rows.  update=False leaves the state as it is (the reference's last
+    iteration, train_coarse.py:134).  Also the path that re-runs a frame h3dgs.coarsestep.GraphedCoarseStep flagged as
+    overflowed.  -> ((loss, l1, ssim) device scalars, radii)"""
+    from .loss import coarse_loss
+    if scene.hier:
+        raise ValueError("coarse_step trains a flat scene (train_coarse.py)")
+    scene.zero_grad()
+    img, radii = render_flat(scene, cam, bg, sh_degree)
+    out = coarse_loss(img, gt, lambda_dssim, mask)
+    out[0].backward()
+    state.update_max_radii(radii)
+    if update:
+        grads = dict(means3D=scene.means3D.grad, shs=scene.shs.grad, opacities=scene.opacities.grad, scales=scene.scales.grad,
+                     rotations=scene.rotations.grad)
+        state.param_step(scene, {k: v.contiguous() for k, v in grads.items()}, cameras_extent)
+    return out, radii
+
+
 def fov_threshold(tau, cam):
     """render_hierarchy.py:55-56"""
     return (2 * (tau + 0.5)) * cam.tanfovx / (0.5 * cam.W)

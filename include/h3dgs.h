@@ -306,7 +306,8 @@ int h3dgs_invdepth_l1_grad(int32_t H, int32_t W, const float* invdepth, const fl
  *   n = sqrtf(x*x + y*y) of dL_dmeans2D[i] ([P,3]; both products, the sum and the root rounded to fp32, no FMA);
  *   denom[i] += 1.  The maxima propagate NaN as torch.max.
  * scan_info (h3dgs_state_view.scan_info of a capacity-mode frame) or NULL: when scan_info[2] is set nothing is changed --
- * an overflowed frame has the radii of the real frame but zero gradients, and the caller re-runs it in exact mode. */
+ * an overflowed frame has the radii of the real frame but zero gradients, and the caller re-runs it in exact mode.
+ * xyz_gradient_accum and denom may both be NULL (train_coarse keeps max_radii2D only); dL_dmeans2D is then unused. */
 int h3dgs_densify_stats(int32_t P, const int32_t* radii, const float* dL_dmeans2D, float* max_radii2D,
                         float* xyz_gradient_accum, float* denom, const uint32_t* scan_info, void* stream);
 /* Status words of the sync-free train_single step, written by one device thread: out[0] = loss = photo + weight * depth,
@@ -463,10 +464,62 @@ int h3dgs_merge_hierarchies(int32_t K, const int64_t* node_offsets, const int64_
 /* ---- sparse Adam (SURVEY.md 8f-4; replaces scene/OurAdam.py:249-337 as driven by train_single.py:170-178) ----
  * In-place Adam update of the rows listed in relevant[num_relevant] (int64 row indices) of one parameter
  * tensor viewed as [rows, width]; `step` is the 1-based step count of that tensor (the reference
- * increments it on every call, whatever the rows).  amsgrad off, weight_decay 0, minimise. */
+ * increments it on every call, whatever the rows).  amsgrad off, weight_decay 0, minimise.  A negative entry of
+ * relevant is skipped; relevant == NULL updates rows [0, num_relevant) (OurAdam's dense step for an empty index). */
 int h3dgs_sparse_adam(int64_t num_relevant, int32_t width, const int64_t* relevant, float* param, const float* grad,
                       float* exp_avg, float* exp_avg_sq, double lr, double beta1, double beta2, double eps, int64_t step,
                       void* stream);
+
+/* ---- train_coarse's objective and parameter step (train_coarse.py:97-145, render_coarse at gaussian_renderer/__init__.py:296-407) ----
+ * The coarse loss is the post-loss pair above without exposure and without clamp: a_c = y_c * mask (mask a DEVICE [H,W]
+ * or NULL = ones), sums / maps as h3dgs_post_loss_forward, and
+ *   dL_dimg_c = mask * (coeffs[0] sign(a_c - gt_c) + coeffs[1] d(sum ssim)/d a_c)
+ * for every y (render_coarse's image is clamped only below, so y > 1 occurs and passes its gradient).  With a mask of
+ * ones and img in [0, 1] both equal h3dgs_l1_ssim_forward / _backward with C = 3, bit for bit. */
+int h3dgs_coarse_loss_forward(int32_t H, int32_t W, const float* img, const float* gt, const float* mask, double* sums,
+                              float* maps, void* stream);
+int h3dgs_coarse_loss_backward(int32_t H, int32_t W, const float* img, const float* gt, const float* mask, const float* maps,
+                               const float* coeffs, float* dL_dimg, void* stream);
+/* Status words of the sync-free coarse step, written by one device thread: out[0] = loss, out[1] = L1, out[2] = SSIM (as
+ * h3dgs_post_step_status), out[3..5] = scan_info[0..2] (D, longest tile list, binning overflow). */
+int h3dgs_coarse_step_status(const double* sums, double inv_numel, double lambda_dssim, const uint32_t* scan_info,
+                             double* out, void* stream);
+
+/* The parameter side of one train_coarse iteration (csrc/coarse_param.cu).  GaussianModel's six stored tensors, group
+ * order of training_setup: 0 _xyz [N,3], 1 _features_dc [N,1,3], 2 _features_rest [N,sh_coeffs-1,3], 3 _opacity [N,1],
+ * 4 _scaling [N,3], 5 _rotation [N,4]; exp_avg / exp_avg_sq alike; `step` a DEVICE int64, the Adam steps taken so far
+ * (OurAdam's state["step"], equal for the six).  The activated rows the rasterizer reads -- means3D [N,3], shs
+ * [N,sh_coeffs,3], opacities [N], scales [N,3], rotations [N,4] -- are written here, and their gradients (the rasterizer
+ * backward's full-size output) are read.  scratch: H3DGS_COARSE_SCRATCH_BYTES of device memory.
+ * mode H3DGS_COARSE_STEP, per row in the reference's order: the activations' backward to the stored gradients (sigmoid
+ *   as (g * (1 - y)) * y on the activated opacity, exp as g * y on the activated scale, F.normalize's backward), the
+ *   scaling gradient zeroed for rows < skybox_points, relevance = stored opacity gradient != 0 (NaN counts), Adam
+ *   (adam.cuh arithmetic, bias corrections of step + 1 formed on the device in double) on the relevant rows and on row 0
+ *   whenever any row is relevant (the zero column of the unflattened nonzero() index), on EVERY row when none is (OurAdam's
+ *   dense step for an empty index), step += 1 always, then for rows
+ *   >= skybox_points whose largest exp(_scaling) exceeds rescale_threshold (float32(cameras_extent * 0.1)) _scaling =
+ *   log(exp(_scaling) * 0.8f), and the activations of every row that changed.  scan_info (NULL = exact mode) with
+ *   scan_info[2] set: nothing at all is changed.  No host synchronisation.
+ * mode H3DGS_COARSE_ACTIVATE: only the activations of every row (grads, moments, step and scratch unused).
+ * mode H3DGS_COARSE_BIAS: only the prologue: scratch receives float step_size[6] = (float)(lr / (1 - beta1^(step+1))),
+ *   then float bc2_sqrt[6] = (float)sqrt(1 - beta2^(step+1)). */
+#define H3DGS_COARSE_SCRATCH_BYTES 64
+enum { H3DGS_COARSE_STEP = 0, H3DGS_COARSE_ACTIVATE = 1, H3DGS_COARSE_BIAS = 2 };
+typedef struct h3dgs_coarse_args {
+    int32_t N, sh_coeffs, skybox_points;
+    float rescale_threshold;
+    float* params[6];
+    float* exp_avg[6];
+    float* exp_avg_sq[6];
+    double lr[6], beta1[6], beta2[6], eps[6];
+    int64_t* step;
+    void* scratch;
+    const float* grad_means3D; const float* grad_shs; const float* grad_opacities; const float* grad_scales;
+    const float* grad_rotations;
+    float* means3D; float* shs; float* opacities; float* scales; float* rotations;
+    const uint32_t* scan_info;
+} h3dgs_coarse_args;
+int h3dgs_coarse_param_step(const h3dgs_coarse_args* args, int32_t mode, void* stream);
 
 /* ---- per-stage device timing (bench.py roofline) ----
  * When enabled, every stage launch is bracketed by two cudaEvents recorded on the stream
