@@ -23,6 +23,7 @@ KIDS_MAX = 65535
 TILE = 16
 U = 2.0 ** -24                               # fp32 unit roundoff
 MARGIN = 1e-5                                # smallest relative decision margin
+PAIRS_PER_CHUNK = 1 << 17
 
 # ---- error analysis (fp32 + MUFU), relative errors -------------------------------------------------------------------
 # exponent: power = (C d + B) d + A in fp32 carries a few ulp of the magnitude of its terms, mag = |A| + |B d| + |C d^2|
@@ -88,117 +89,130 @@ def blend_reference(records, ranges, point_list, W, H, bg, dL_dcolor=None, dL_di
         gdep = np.asarray(dL_dinvdepth, np.float64).reshape(H, W) if (do_depth and dL_dinvdepth is not None) else None
     for tile in range(ranges.shape[0]):
         tx, ty = tile % gx, tile // gx
-        ys, xs = np.meshgrid(np.arange(ty * TILE, min(ty * TILE + TILE, H)), np.arange(tx * TILE, min(tx * TILE + TILE, W)),
-                             indexing="ij")
-        ys, xs = ys.ravel(), xs.ravel()
+        ys_t, xs_t = np.meshgrid(np.arange(ty * TILE, min(ty * TILE + TILE, H)), np.arange(tx * TILE, min(tx * TILE + TILE, W)),
+                                 indexing="ij")
+        ys_t, xs_t = ys_t.ravel(), xs_t.ravel()
         s, e = ranges[tile]
-        if ys.size == 0:
+        if ys_t.size == 0:
             continue
         if e <= s:
             for c in range(3):
-                out["color"][c, ys, xs] = bg[c]
+                out["color"][c, ys_t, xs_t] = bg[c]
             continue
         ids = point_list[s:e]
-        R = rec[ids]
-        x, y, cx, cy, cz, op, t, rgb, invd = R[:, 0], R[:, 1], R[:, 2], R[:, 3], R[:, 4], R[:, 5], R[:, 6], R[:, 8:11], R[:, 11]
-        dx = x[None] - xs[:, None]
-        dy = y[None] - ys[:, None]
-        power = -0.5 * (cx * dx * dx + cz * dy * dy) - cy * dx * dy
-        mag = 0.5 * (np.abs(cx) * dx * dx + np.abs(cz) * dy * dy) + np.abs(cy * dx * dy)
-        G = np.exp(power)
-        araw = op * G
-        ab = np.minimum(ALPHA_CAP, araw)
-        if hier:
-            al, dadb, act = hier_weight(ab, t[None], kids[ids][None])
-        else:
-            al, dadb, act = ab, np.ones_like(ab), np.zeros_like(ab, bool)
-        eps_a = 4 * U * mag + EPS_EX2 + 3 * U + np.where(act, EPS_HIER, 0.0)
-        valid = (power <= 0) & (al >= ALPHA_SKIP)
-        aeff = np.where(valid, al, 0.0)
-        Tall = np.cumprod(1 - aeff, axis=1)
-        contrib = valid & (Tall >= T_STOP)
-        a_c = np.where(contrib, al, 0.0)
-        Tafter = np.cumprod(1 - a_c, axis=1)
-        Tbefore = np.concatenate([np.ones((xs.size, 1)), Tafter[:, :-1]], 1)
-        Tfin = Tafter[:, -1]
-        n = ids.size
-        pos = np.arange(1, n + 1)
-        last = np.where(contrib, pos[None], 0).max(1)
-        w = a_c * Tbefore
-        # T's relative error in front of each entry, and at the end
-        tstep = np.where(contrib, U + eps_a * a_c / (1 - a_c), 0.0)
-        kap_before = np.concatenate([np.zeros((xs.size, 1)), np.cumsum(tstep, 1)[:, :-1]], 1)
-        kap = tstep.sum(1)
-        # decisions: pairs up to the stopping entry (or the end of the list) are the ones that matter
-        stop_pos = np.where((valid & ~contrib).any(1), np.argmax(valid & ~contrib, 1), n - 1)
-        rel = pos[None] - 1 <= stop_pos[:, None]
-        m = np.maximum(MARGIN, 4 * eps_a)
-        near_pw = rel & (power != 0) & (np.abs(power) <= MARGIN * mag)
-        near_sk = rel & (power <= 0) & (np.abs(al - ALPHA_SKIP) <= m * ALPHA_SKIP)
-        near_cap = rel & (power <= 0) & (np.abs(araw - ALPHA_CAP) <= m * ALPHA_CAP)
-        mT = np.maximum(MARGIN, 4 * (kap_before + eps_a * al / np.maximum(1 - al, 1e-3)))
-        near_st = rel & valid & (np.abs(Tbefore * (1 - al) - T_STOP) <= mT * T_STOP)
-        near = near_pw | near_sk | near_cap | near_st
-        for kname, arr in (("power", near_pw), ("skip", near_sk), ("cap", near_cap), ("stop", near_st)):
-            out["near_kind"][kname] += int(arr.any(1).sum())
-        npx = near.any(1)
-        out["near_pixel"][ys[npx], xs[npx]] = True
-        if npx.any():
-            hit = (valid | near_sk)[npx].any(0)
-            out["near_gauss"][ids[hit]] = True
-
-        e_pair = 2 * kap[:, None] + 2 * eps_a + 16 * U           # relative error budget of one pair's terms
-        col = w @ rgb + Tfin[:, None] * bg[None]
-        out["color"][:, ys, xs] = col.T
-        out["color_tol"][ys, xs] = 2 * ((w * e_pair) @ np.abs(rgb).max(1) + Tfin * np.abs(bg).max() * (kap + U)) + 1e-12
-        out["final_T"][ys, xs] = Tfin
-        out["final_T_tol"][ys, xs] = 2 * Tfin * (kap + U) + 1e-30
-        out["invdepth"][ys, xs] = w @ invd
-        out["invdepth_tol"][ys, xs] = 2 * ((w * e_pair) @ np.abs(invd)) + 1e-12
-        out["n_contrib"][ys, xs] = last
-        if not backward:
-            continue
-        gc = gcol[:, ys, xs].T                                   # [m][3]
-        cg = rgb @ gc.T                                          # [n][m] -> transposed below
-        cg = cg.T
-        cg_abs = np.abs(rgb) @ np.abs(gc).T
-        cg_abs = cg_abs.T
-        if gdep is not None:
-            gd = gdep[ys, xs]
-            cg = cg + invd[None] * gd[:, None]
-            cg_abs = cg_abs + np.abs(invd)[None] * np.abs(gd)[:, None]
-        bgd = gc @ bg
-        wcg = w * cg
-        behind = np.cumsum(wcg[:, ::-1], 1)[:, ::-1] - wcg        # sum over the contributors behind each entry
-        behind_abs = np.cumsum((w * cg_abs)[:, ::-1], 1)[:, ::-1] - w * cg_abs
-        om = np.where(contrib, 1 - a_c, 1.0)
-        dL_da = np.where(contrib, Tbefore * cg - (behind + Tfin[:, None] * bgd[:, None]) / om, 0.0)
-        dL_da_abs = np.where(contrib, Tbefore * cg_abs + (behind_abs + Tfin[:, None] * np.abs(bgd)[:, None]) / om, 0.0)
-        dL_dab, dL_dab_abs = dL_da * dadb, dL_da_abs * np.abs(dadb)
-        p, p_abs = G * dL_dab, G * dL_dab_abs
-        o = op[None]
-        terms = [
-            (o * p * -(cx * dx + cy * dy), o * p_abs * (np.abs(cx * dx) + np.abs(cy * dy))),
-            (o * p * -(cy * dx + cz * dy), o * p_abs * (np.abs(cy * dx) + np.abs(cz * dy))),
-            (o * p * dx * dx, o * p_abs * dx * dx),
-            (o * p * dx * dy, o * p_abs * np.abs(dx * dy)),
-            (o * p * dy * dy, o * p_abs * dy * dy),
-            (p, p_abs),
-        ]
-        for c in range(3):
-            terms.append((w * gc[:, c:c + 1], w * np.abs(gc[:, c:c + 1])))
-        if gdep is not None:
-            terms.append((w * gd[:, None], w * np.abs(gd[:, None])))
-        npix = contrib.sum(0)
-        np.add.at(npix_of, ids, npix)
-        for col_i, (v, va) in enumerate(terms):
-            np.add.at(out["accum"][:, col_i], ids, v.sum(0))
-            np.add.at(out["accum_abs"][:, col_i], ids, va.sum(0))
-            np.add.at(out["accum_tol"][:, col_i], ids, (va * e_pair).sum(0))
+        # the tile's pixels in chunks of about PAIRS_PER_CHUNK (pixel, entry) pairs: a deep list does not hold its ~40
+        # [pixels x entries] float64 arrays for all 256 pixels at once.  Per pixel the decisions are the same and the
+        # values differ by the float64 rounding of the matrix products only; the per-Gaussian sums add the chunks'
+        # partial sums in another order.
+        step = int(np.clip(PAIRS_PER_CHUNK // ids.size, 1, ys_t.size))
+        for c0 in range(0, ys_t.size, step):
+            ys, xs = ys_t[c0:c0 + step], xs_t[c0:c0 + step]
+            _blend_pixels(out, rec, ids, xs, ys, kids, bg, hier, npix_of, gcol if backward else None,
+                          gdep if backward else None)
     # the per-Gaussian sums are fp32 additions of up to npix terms (span reductions, then atomics in any order)
     out["accum_tol"] = 2 * out["accum_tol"] + (8 + npix_of)[:, None] * U * out["accum_abs"] + 1e-30
     out["npix"] = npix_of
     return out
+
+
+def _blend_pixels(out, rec, ids, xs, ys, kids, bg, hier, npix_of, gcol, gdep):
+    """blend_reference's work for the pixels (xs, ys) of one tile over its list ids, written into `out`"""
+    R = rec[ids]
+    x, y, cx, cy, cz, op, t, rgb, invd = R[:, 0], R[:, 1], R[:, 2], R[:, 3], R[:, 4], R[:, 5], R[:, 6], R[:, 8:11], R[:, 11]
+    dx = x[None] - xs[:, None]
+    dy = y[None] - ys[:, None]
+    power = -0.5 * (cx * dx * dx + cz * dy * dy) - cy * dx * dy
+    mag = 0.5 * (np.abs(cx) * dx * dx + np.abs(cz) * dy * dy) + np.abs(cy * dx * dy)
+    G = np.exp(power)
+    araw = op * G
+    ab = np.minimum(ALPHA_CAP, araw)
+    if hier:
+        al, dadb, act = hier_weight(ab, t[None], kids[ids][None])
+    else:
+        al, dadb, act = ab, np.ones_like(ab), np.zeros_like(ab, bool)
+    eps_a = 4 * U * mag + EPS_EX2 + 3 * U + np.where(act, EPS_HIER, 0.0)
+    valid = (power <= 0) & (al >= ALPHA_SKIP)
+    aeff = np.where(valid, al, 0.0)
+    Tall = np.cumprod(1 - aeff, axis=1)
+    contrib = valid & (Tall >= T_STOP)
+    a_c = np.where(contrib, al, 0.0)
+    Tafter = np.cumprod(1 - a_c, axis=1)
+    Tbefore = np.concatenate([np.ones((xs.size, 1)), Tafter[:, :-1]], 1)
+    Tfin = Tafter[:, -1]
+    n = ids.size
+    pos = np.arange(1, n + 1)
+    last = np.where(contrib, pos[None], 0).max(1)
+    w = a_c * Tbefore
+    # T's relative error in front of each entry, and at the end
+    tstep = np.where(contrib, U + eps_a * a_c / (1 - a_c), 0.0)
+    kap_before = np.concatenate([np.zeros((xs.size, 1)), np.cumsum(tstep, 1)[:, :-1]], 1)
+    kap = tstep.sum(1)
+    # decisions: pairs up to the stopping entry (or the end of the list) are the ones that matter
+    stop_pos = np.where((valid & ~contrib).any(1), np.argmax(valid & ~contrib, 1), n - 1)
+    rel = pos[None] - 1 <= stop_pos[:, None]
+    m = np.maximum(MARGIN, 4 * eps_a)
+    near_pw = rel & (power != 0) & (np.abs(power) <= MARGIN * mag)
+    near_sk = rel & (power <= 0) & (np.abs(al - ALPHA_SKIP) <= m * ALPHA_SKIP)
+    near_cap = rel & (power <= 0) & (np.abs(araw - ALPHA_CAP) <= m * ALPHA_CAP)
+    mT = np.maximum(MARGIN, 4 * (kap_before + eps_a * al / np.maximum(1 - al, 1e-3)))
+    near_st = rel & valid & (np.abs(Tbefore * (1 - al) - T_STOP) <= mT * T_STOP)
+    near = near_pw | near_sk | near_cap | near_st
+    for kname, arr in (("power", near_pw), ("skip", near_sk), ("cap", near_cap), ("stop", near_st)):
+        out["near_kind"][kname] += int(arr.any(1).sum())
+    npx = near.any(1)
+    out["near_pixel"][ys[npx], xs[npx]] = True
+    if npx.any():
+        hit = (valid | near_sk)[npx].any(0)
+        out["near_gauss"][ids[hit]] = True
+
+    e_pair = 2 * kap[:, None] + 2 * eps_a + 16 * U           # relative error budget of one pair's terms
+    col = w @ rgb + Tfin[:, None] * bg[None]
+    out["color"][:, ys, xs] = col.T
+    out["color_tol"][ys, xs] = 2 * ((w * e_pair) @ np.abs(rgb).max(1) + Tfin * np.abs(bg).max() * (kap + U)) + 1e-12
+    out["final_T"][ys, xs] = Tfin
+    out["final_T_tol"][ys, xs] = 2 * Tfin * (kap + U) + 1e-30
+    out["invdepth"][ys, xs] = w @ invd
+    out["invdepth_tol"][ys, xs] = 2 * ((w * e_pair) @ np.abs(invd)) + 1e-12
+    out["n_contrib"][ys, xs] = last
+    if gcol is None:
+        return
+    gc = gcol[:, ys, xs].T                                   # [m][3]
+    cg = rgb @ gc.T                                          # [n][m] -> transposed below
+    cg = cg.T
+    cg_abs = np.abs(rgb) @ np.abs(gc).T
+    cg_abs = cg_abs.T
+    if gdep is not None:
+        gd = gdep[ys, xs]
+        cg = cg + invd[None] * gd[:, None]
+        cg_abs = cg_abs + np.abs(invd)[None] * np.abs(gd)[:, None]
+    bgd = gc @ bg
+    wcg = w * cg
+    behind = np.cumsum(wcg[:, ::-1], 1)[:, ::-1] - wcg        # sum over the contributors behind each entry
+    behind_abs = np.cumsum((w * cg_abs)[:, ::-1], 1)[:, ::-1] - w * cg_abs
+    om = np.where(contrib, 1 - a_c, 1.0)
+    dL_da = np.where(contrib, Tbefore * cg - (behind + Tfin[:, None] * bgd[:, None]) / om, 0.0)
+    dL_da_abs = np.where(contrib, Tbefore * cg_abs + (behind_abs + Tfin[:, None] * np.abs(bgd)[:, None]) / om, 0.0)
+    dL_dab, dL_dab_abs = dL_da * dadb, dL_da_abs * np.abs(dadb)
+    p, p_abs = G * dL_dab, G * dL_dab_abs
+    o = op[None]
+    terms = [
+        (o * p * -(cx * dx + cy * dy), o * p_abs * (np.abs(cx * dx) + np.abs(cy * dy))),
+        (o * p * -(cy * dx + cz * dy), o * p_abs * (np.abs(cy * dx) + np.abs(cz * dy))),
+        (o * p * dx * dx, o * p_abs * dx * dx),
+        (o * p * dx * dy, o * p_abs * np.abs(dx * dy)),
+        (o * p * dy * dy, o * p_abs * dy * dy),
+        (p, p_abs),
+    ]
+    for c in range(3):
+        terms.append((w * gc[:, c:c + 1], w * np.abs(gc[:, c:c + 1])))
+    if gdep is not None:
+        terms.append((w * gd[:, None], w * np.abs(gd[:, None])))
+    npix = contrib.sum(0)
+    np.add.at(npix_of, ids, npix)
+    for col_i, (v, va) in enumerate(terms):
+        np.add.at(out["accum"][:, col_i], ids, v.sum(0))
+        np.add.at(out["accum_abs"][:, col_i], ids, va.sum(0))
+        np.add.at(out["accum_tol"][:, col_i], ids, (va * e_pair).sum(0))
 
 
 def compare(got, want, tol, mask=None):

@@ -22,3 +22,15 @@ def test_gpu_parity_files_pass_on_the_emulator():
     assert r.returncode == 0, tail + r.stderr[-1500:]
     m = re.search(r"(\d+) passed", tail)
     assert m and int(m.group(1)) >= 70 and "failed" not in tail, tail
+
+
+def test_gpu_blend_deep_passes_on_the_emulator():
+    """The deep tile lists (every tile-sort class up to 8192 entries, the radix sort beyond, walls at every batch edge)
+    in their flat and hierarchy variants; the inverse-depth variants only add the tenth sum and are left to the GPU."""
+    env = dict(os.environ, H3DGS_EMULATE="1")
+    r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_blend_deep.py", "-q", "-p", "no:cacheprovider",
+                        "-k", "not depth"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
+    tail = r.stdout[-1500:]
+    assert r.returncode == 0, tail + r.stderr[-1500:]
+    m = re.search(r"(\d+) passed", tail)
+    assert m and int(m.group(1)) >= 6 and "failed" not in tail, tail
