@@ -21,117 +21,13 @@
 // pass that raises the any-relevant word (8 bytes per row), and the update pass over every row, whose row set the word
 // selects.  An overflowed capacity-mode frame (scan_info[2]) changes nothing.
 #include "common.cuh"
-#include "adam.cuh"
+#include "param_row.cuh"
 
 namespace h3dgs {
 
-struct CoarseScratch { float step_size[6], bc2_sqrt[6]; int any; };
 static_assert(sizeof(CoarseScratch) <= H3DGS_COARSE_SCRATCH_BYTES, "scratch");
 
-struct CoarseConst { float beta1[6], beta2[6], omb1[6], omb2[6], eps[6]; double lr[6], beta1d[6], beta2d[6]; };
-
 __device__ __forceinline__ bool overflowed(const h3dgs_coarse_args& a) { return a.scan_info && a.scan_info[2]; }
-
-__device__ __forceinline__ float sigmoid_f(float x) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x))); }
-
-// |q| as the forward and the backward take it, and the clamp_min(1e-12) divisor (NaN propagates as torch.clamp_min)
-__device__ __forceinline__ void quat_norm(const float q[4], float& n, float& d)
-{
-    n = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q[0], q[0]), __fmul_rn(q[1], q[1])), __fmul_rn(q[2], q[2])),
-                             __fmul_rn(q[3], q[3])));
-    d = (n != n || n > 1e-12f) ? n : 1e-12f;
-}
-
-__device__ __forceinline__ void write_activated(const h3dgs_coarse_args& a, int i, const float s[3], const float e[3], const float q[4])
-{
-    const size_t M3 = (size_t)a.sh_coeffs * 3;
-#pragma unroll
-    for (int c = 0; c < 3; c++) a.means3D[3 * (size_t)i + c] = a.params[0][3 * (size_t)i + c];
-#pragma unroll
-    for (int c = 0; c < 3; c++) a.shs[M3 * i + c] = a.params[1][3 * (size_t)i + c];
-    for (int j = 0; j < (int)M3 - 3; j++) a.shs[M3 * i + 3 + j] = a.params[2][(M3 - 3) * i + j];
-    a.opacities[i] = sigmoid_f(a.params[3][i]);
-#pragma unroll
-    for (int c = 0; c < 3; c++) a.scales[3 * (size_t)i + c] = e[c];
-    float n, d;
-    quat_norm(q, n, d);
-#pragma unroll
-    for (int c = 0; c < 4; c++) a.rotations[4 * (size_t)i + c] = __fdiv_rn(q[c], d);
-}
-
-// the row's scaling after the step and the rescale, exp of it, and the activations when anything changed
-__device__ __forceinline__ void rescale_and_activate(const h3dgs_coarse_args& a, int i, bool changed)
-{
-    float s[3], e[3], q[4];
-#pragma unroll
-    for (int c = 0; c < 3; c++) { s[c] = a.params[4][3 * (size_t)i + c]; e[c] = expf(s[c]); }
-    if (i >= a.skybox_points) {
-        float mx = e[0];
-#pragma unroll
-        for (int c = 1; c < 3; c++) mx = (mx != mx) ? mx : ((e[c] != e[c] || e[c] > mx) ? e[c] : mx);
-        if (mx > a.rescale_threshold) {
-#pragma unroll
-            for (int c = 0; c < 3; c++) {
-                s[c] = logf(__fmul_rn(e[c], 0.8f));
-                a.params[4][3 * (size_t)i + c] = s[c];
-                e[c] = expf(s[c]);
-            }
-            changed = true;
-        }
-    }
-    if (!changed) return;
-#pragma unroll
-    for (int c = 0; c < 4; c++) q[c] = a.params[5][4 * (size_t)i + c];
-    write_activated(a, i, s, e, q);
-}
-
-__device__ __forceinline__ void adam_at(const h3dgs_coarse_args& a, const CoarseConst& k, const CoarseScratch& sc, int grp,
-                                        size_t o, float g)
-{
-    float p = a.params[grp][o], m = a.exp_avg[grp][o], v = a.exp_avg_sq[grp][o];
-    adam_element(p, g, m, v, k.beta1[grp], k.beta2[grp], k.omb1[grp], k.omb2[grp], sc.step_size[grp], sc.bc2_sqrt[grp], k.eps[grp]);
-    a.params[grp][o] = p;
-    a.exp_avg[grp][o] = m;
-    a.exp_avg_sq[grp][o] = v;
-}
-
-// Adam on every stored element of row i, with the stored opacity gradient go already formed
-__device__ __forceinline__ void adam_row(const h3dgs_coarse_args& a, const CoarseConst& k, const CoarseScratch& sc, int i, float go)
-{
-    const size_t M3 = (size_t)a.sh_coeffs * 3;
-#pragma unroll
-    for (int c = 0; c < 3; c++) adam_at(a, k, sc, 0, 3 * (size_t)i + c, a.grad_means3D[3 * (size_t)i + c]);
-#pragma unroll
-    for (int c = 0; c < 3; c++) adam_at(a, k, sc, 1, 3 * (size_t)i + c, a.grad_shs[M3 * i + c]);
-    for (int j = 0; j < (int)M3 - 3; j++) adam_at(a, k, sc, 2, (M3 - 3) * i + j, a.grad_shs[M3 * i + 3 + j]);
-    adam_at(a, k, sc, 3, (size_t)i, go);
-    const bool locked = i < a.skybox_points;
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-        const size_t o = 3 * (size_t)i + c;
-        adam_at(a, k, sc, 4, o, locked ? 0.f : __fmul_rn(a.grad_scales[o], a.scales[o]));
-    }
-    // F.normalize's backward: x / clamp_min(norm(x), 1e-12).  div: g / d to x, -g * ((x / d) / d) summed to d;
-    // clamp_min passes where norm >= 1e-12; norm: x * (grad / norm), 0 where norm == 0
-    float q[4], g[4];
-#pragma unroll
-    for (int c = 0; c < 4; c++) { q[c] = a.params[5][4 * (size_t)i + c]; g[c] = a.grad_rotations[4 * (size_t)i + c]; }
-    float n, d;
-    quat_norm(q, n, d);
-    float gd = 0.f;
-#pragma unroll
-    for (int c = 0; c < 4; c++) gd = __fadd_rn(gd, __fmul_rn(-g[c], __fdiv_rn(__fdiv_rn(q[c], d), d)));
-    if (!(n >= 1e-12f)) gd = 0.f;
-    const float t = n == 0.f ? 0.f : __fdiv_rn(gd, n);
-#pragma unroll
-    for (int c = 0; c < 4; c++) adam_at(a, k, sc, 5, 4 * (size_t)i + c, __fadd_rn(__fdiv_rn(g[c], d), __fmul_rn(q[c], t)));
-}
-
-__device__ __forceinline__ float stored_opacity_grad(const h3dgs_coarse_args& a, int i)
-{
-    const float y = a.opacities[i];
-    return __fmul_rn(__fmul_rn(a.grad_opacities[i], __fsub_rn(1.f, y)), y);        // sigmoid_backward: g * (1 - y) * y
-}
 
 // count = 1 (H3DGS_COARSE_STEP): the step is taken, step += 1 first (OurAdam's step_t += 1 of every call, whatever the
 // rows, scene/OurAdam.py:277, 359); the bias corrections are those of the new count
@@ -141,11 +37,7 @@ __global__ void coarse_prologue_kernel(h3dgs_coarse_args a, CoarseConst k, int c
     CoarseScratch* sc = (CoarseScratch*)a.scratch;
     const double step = (double)(*a.step + 1);
     if (count) *a.step += 1;
-    for (int g = 0; g < 6; g++) {
-        const double bc1 = 1.0 - pow(k.beta1d[g], step), bc2 = 1.0 - pow(k.beta2d[g], step);
-        sc->step_size[g] = (float)(k.lr[g] / bc1);
-        sc->bc2_sqrt[g] = (float)sqrt(bc2);
-    }
+    for (int g = 0; g < 6; g++) bias_corrections(k.lr[g], k.beta1d[g], k.beta2d[g], step, sc->step_size[g], sc->bc2_sqrt[g]);
     sc->any = 0;
 }
 
@@ -167,8 +59,8 @@ __global__ void __launch_bounds__(256) coarse_update_kernel(h3dgs_coarse_args a,
     const CoarseScratch& sc = *(const CoarseScratch*)a.scratch;
     const float go = stored_opacity_grad(a, i);
     const bool update = sc.any ? (go != 0.f || i == 0) : true;
-    if (update) adam_row(a, k, sc, i, go);
-    rescale_and_activate(a, i, update);
+    if (update) adam_row(a, k, sc, i, go, i < a.skybox_points);
+    rescale_and_activate(a, i, update, a.skybox_points);
 }
 
 __global__ void __launch_bounds__(256) coarse_activate_kernel(h3dgs_coarse_args a)

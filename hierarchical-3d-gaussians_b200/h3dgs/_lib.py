@@ -73,6 +73,20 @@ class CoarseArgs(C.Structure):
     ]
 
 
+SINGLE_SCRATCH_BYTES = 64     # H3DGS_SINGLE_SCRATCH_BYTES
+SINGLE_STEP, SINGLE_NO_GAUSSIAN_STEP, SINGLE_EXPOSURE_ROW, SINGLE_BIAS = 0, 1, 2, 3
+
+
+class SingleArgs(C.Structure):
+    """struct h3dgs_single_args"""
+    _fields_ = [
+        ("gauss", CoarseArgs), ("skybox_locked", C.c_int32), ("scaffold_points", C.c_int32), ("n_images", C.c_int32),
+        ("lrs", C.c_void_p), ("exposure", C.c_void_p), ("exposure_exp_avg", C.c_void_p), ("exposure_exp_avg_sq", C.c_void_p),
+        ("exposure_step", C.c_void_p), ("exposure_beta1", C.c_double), ("exposure_beta2", C.c_double),
+        ("exposure_eps", C.c_double), ("exposure_grad", C.c_void_p), ("image_index", C.c_void_p), ("exposure_row", C.c_void_p),
+    ]
+
+
 class StateView(C.Structure):
     """struct h3dgs_state_view"""
     _fields_ = [(n, C.c_void_p) for n in ("depths", "tiles_touched", "point_offsets", "records", "keys_sorted",
@@ -179,6 +193,9 @@ def bind(l):
     if hasattr(l, "h3dgs_coarse_param_step"):    # train_coarse's parameter step (an emulation build has it when it compiles coarse_param.cu)
         l.h3dgs_coarse_param_step.restype = C.c_int
         l.h3dgs_coarse_param_step.argtypes = [C.POINTER(CoarseArgs), C.c_int32, C.c_void_p]
+    if hasattr(l, "h3dgs_single_param_step"):    # train_single's parameter step (likewise)
+        l.h3dgs_single_param_step.restype = C.c_int
+        l.h3dgs_single_param_step.argtypes = [C.POINTER(SingleArgs), C.c_int32, C.c_void_p]
     l.h3dgs_invdepth_l1_grad.restype = C.c_int
     l.h3dgs_invdepth_l1_grad.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
     l.h3dgs_densify_stats.restype = C.c_int

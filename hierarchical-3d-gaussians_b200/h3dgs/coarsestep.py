@@ -77,9 +77,9 @@ class CoarseState:
         self.scratch = torch.zeros(_lib.COARSE_SCRATCH_BYTES, dtype=torch.uint8, device=dev)
 
     # ---- GaussianModel / OurAdam interchange ----------------------------------------------
-    @classmethod
-    def from_model(cls, gaussians):
-        """from a GaussianModel after training_setup (and the xyz lr set to 0), with its OurAdam's state if it has any"""
+    @staticmethod
+    def _model_groups(gaussians):
+        """-> (params, lrs, betas, eps, exp_avg or None, exp_avg_sq or None, step) of a GaussianModel and its OurAdam"""
         params = [getattr(gaussians, a) for a in _MODEL_ATTRS]
         opt = gaussians.optimizer
         groups = {g["name"]: g for g in opt.param_groups}
@@ -89,9 +89,14 @@ class CoarseState:
         steps = {int(float(s["step"])) for s in st} if have else {0}
         if len(steps) != 1:
             raise ValueError(f"the six groups have taken different step counts {sorted(steps)}")
-        return cls(params, gaussians.skybox_points, [g["lr"] for g in gs], [tuple(g["betas"]) for g in gs],
-                   [g["eps"] for g in gs], [s["exp_avg"] for s in st] if have else None,
-                   [s["exp_avg_sq"] for s in st] if have else None, steps.pop(),
+        return (params, [g["lr"] for g in gs], [tuple(g["betas"]) for g in gs], [g["eps"] for g in gs],
+                [s["exp_avg"] for s in st] if have else None, [s["exp_avg_sq"] for s in st] if have else None, steps.pop())
+
+    @classmethod
+    def from_model(cls, gaussians):
+        """from a GaussianModel after training_setup (and the xyz lr set to 0), with its OurAdam's state if it has any"""
+        params, lrs, betas, eps, m, v, step = cls._model_groups(gaussians)
+        return cls(params, gaussians.skybox_points, lrs, betas, eps, m, v, step,
                    getattr(gaussians, "max_radii2D", None) if getattr(gaussians, "max_radii2D", None) is not None and
                    gaussians.max_radii2D.numel() == params[0].shape[0] else None)
 

@@ -33,6 +33,7 @@ The arithmetic is the one of the exact path: same kernels, same order, so images
 bit-identical to pipeline.l1_step(fused=True) whenever the frame fits.
 """
 import ctypes as C
+import weakref
 
 import torch
 import torch.distributed as dist
@@ -78,7 +79,11 @@ class GraphedBase:
         self.gt = self.gt_bufs[0]
         self.radii = torch.zeros(self.P, dtype=torch.int32, device=dev)
         self._bufs = [None, None, None]
-        self._alloc_cb = _lib.ALLOC_FN(self._alloc)     # keep the callback object alive
+        # the C-ABI callback reaches this instance through a weak reference: a bound method would make a reference
+        # cycle, and an instance in a cycle is freed only by Python's cycle collector -- whenever it happens to run,
+        # possibly in the middle of another instance's capture
+        me = weakref.ref(self)
+        self._alloc_cb = _lib.ALLOC_FN(lambda user, which, nbytes: me()._alloc(user, which, nbytes))
         self._scan_info = None
         self.graph_a = self.graph_b = None
         self.launches_per_step = 0

@@ -226,17 +226,29 @@ class DensifyStats:
 
 
 def single_step(scene, cam, bg, gt, lambda_dssim=0.2, exposure=None, mask=None, mono_invdepth=None, depth_mask=None,
-                depth_weight=0.0, stats=None, sh_degree=3):
+                depth_weight=0.0, stats=None, sh_degree=3, state=None, cameras_extent=None, update=True):
     """One step of train_single's loop body (train_single.py:94-148) on a flat scene, on the exact path: render() with
     do_depth, the objective (h3dgs.loss.single_loss: exposure, clamp, alpha mask, (1-l) L1 + l (1 - SSIM), plus
     depth_weight times the inverse-depth L1 when mono_invdepth is given and the weight is not 0), backward, and the
     densification statistics into `stats` (a DensifyStats; None skips them).  Gradients land in the scene's tensors and,
     when `exposure` requires grad, in exposure.grad.  Also the path that re-runs a frame
     h3dgs.singlestep.GraphedSingleStep flagged as overflowed.
+
+    state: a h3dgs.singlestep.SingleState (scene = state.make_scene()).  The exposure is then the state's row of the
+    image state.set_image() named, its gradient lands in state.exposure_grad, and with update=True the iteration ends
+    with the state's parameter step (train_single.py:159-186, rescale threshold from cameras_extent), which also
+    refreshes the scene's activated rows.  update=False leaves the state as it is (save, checkpoint, densify and reset
+    iterations, and the last one).
     -> ((loss, photo, l1, ssim, depth_l1) device scalars, radii, means2D with its .grad)"""
     from .loss import single_loss
     if scene.hier:
         raise ValueError("single_step trains a flat scene (train_single.py); a hierarchy goes through post_step")
+    if state is not None:
+        if exposure is not None:
+            raise ValueError("with a state the exposure is the state's row of the frame's image (state.set_image)")
+        if update and cameras_extent is None:
+            raise ValueError("the parameter step needs cameras_extent (the rescale threshold)")
+        exposure = state.exposure_row().requires_grad_(True)
     scene.zero_grad()
     means2D = torch.zeros_like(scene.means3D, requires_grad=True)
     img, radii, invdepth = render_flat(scene, cam, bg, sh_degree, do_depth=True, means2D=means2D)
@@ -244,6 +256,12 @@ def single_step(scene, cam, bg, gt, lambda_dssim=0.2, exposure=None, mask=None, 
     out[0].backward()
     if stats is not None:
         stats.update(radii, means2D.grad)
+    if state is not None:
+        state.exposure_grad.copy_(exposure.grad)
+        if update:
+            grads = dict(means3D=scene.means3D.grad, shs=scene.shs.grad, opacities=scene.opacities.grad,
+                         scales=scene.scales.grad, rotations=scene.rotations.grad)
+            state.param_step(scene, {k: v.contiguous() for k, v in grads.items()}, cameras_extent)
     return out, radii, means2D
 
 

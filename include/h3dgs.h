@@ -521,6 +521,45 @@ typedef struct h3dgs_coarse_args {
 } h3dgs_coarse_args;
 int h3dgs_coarse_param_step(const h3dgs_coarse_args* args, int32_t mode, void* stream);
 
+/* ---- train_single's parameter side (train_single.py:85-88, 157-186; csrc/single_param.cu) ----
+ * gauss: the six stored tensors, their moments, the step count, scratch (H3DGS_SINGLE_SCRATCH_BYTES), the activated
+ * gradients and rows and scan_info, as h3dgs_coarse_args, with these differences:
+ *   gauss.skybox_points  rows the lock covers, and ALL six stored gradients of those rows are 0 when skybox_locked;
+ *   gauss.lr[0]          unused: the xyz lr is lrs[0], a DEVICE double the host fills each iteration (the other five are
+ *                        the constant gauss.lr[1..5]);
+ *   gauss.rescale_threshold  float32(cameras_extent * 0.02); +inf turns the rescale off (--skip_scale_big_gauss).
+ * The rescale covers rows >= scaffold_points (0 = every row).  Relevance is the FLATTENED index: exactly the rows whose
+ * stored opacity gradient is != 0 (NaN counts); with none, OurAdam's dense step on every row.
+ * The exposure: exposure [n_images][3][4] (GaussianModel._exposure) with its torch.optim.Adam moments and DEVICE int64
+ * step count, betas / eps of its one group, lr lrs[1].  Its gradient is exposure_grad [3][4] (fp32) at row
+ * *image_index and 0 elsewhere; every element moves, in the arithmetic of torch.optim.Adam's default CUDA path
+ * (foreach): m = lerp(m, g, 1 - beta1), v = v * beta2 then v + (1 - beta2) * g * g, p + (-lr / bc1) * (m / (sqrt(v) /
+ * sqrt(bc2) + eps)), contracted as torch's kernels are; its bias corrections are formed in double as torch's host floats.
+ * mode H3DGS_SINGLE_STEP: both steps count (step += 1, exposure_step += 1), the exposure Adam, then per row the lock,
+ *   relevance, Adam on the row set, the rescale and the activations of every row that changed.
+ * mode H3DGS_SINGLE_NO_GAUSSIAN_STEP (densify, opacity-reset iterations: the parameters were replaced and carry no
+ *   gradient): exposure_step += 1 and the exposure Adam, then the rescale and the activations; grads, moments and step
+ *   are not touched.
+ * mode H3DGS_SINGLE_EXPOSURE_ROW: exposure_row [3][4] = exposure[*image_index] (the forward's exposure), nothing else.
+ * mode H3DGS_SINGLE_BIAS: only the prologue of a full step (scratch as H3DGS_COARSE_BIAS, then float exposure
+ *   step_size = (float)(-lr / (1 - beta1^(exposure_step+1))) and bc2_sqrt), step counts unchanged.
+ * scan_info[2] set: nothing at all changes -- parameters, both moment sets, both step counts, exposures.
+ * The activation-only pass is h3dgs_coarse_param_step(&gauss, H3DGS_COARSE_ACTIVATE). */
+#define H3DGS_SINGLE_SCRATCH_BYTES 64
+enum { H3DGS_SINGLE_STEP = 0, H3DGS_SINGLE_NO_GAUSSIAN_STEP = 1, H3DGS_SINGLE_EXPOSURE_ROW = 2, H3DGS_SINGLE_BIAS = 3 };
+typedef struct h3dgs_single_args {
+    h3dgs_coarse_args gauss;
+    int32_t skybox_locked, scaffold_points, n_images;
+    const double* lrs;
+    float* exposure; float* exposure_exp_avg; float* exposure_exp_avg_sq;
+    int64_t* exposure_step;
+    double exposure_beta1, exposure_beta2, exposure_eps;
+    const float* exposure_grad;
+    const int32_t* image_index;
+    float* exposure_row;
+} h3dgs_single_args;
+int h3dgs_single_param_step(const h3dgs_single_args* args, int32_t mode, void* stream);
+
 /* ---- per-stage device timing (bench.py roofline) ----
  * When enabled, every stage launch is bracketed by two cudaEvents recorded on the stream
  * the kernel is launched on; h3dgs_profile_read synchronises them and returns the summed
