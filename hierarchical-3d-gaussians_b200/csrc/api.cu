@@ -105,6 +105,20 @@ int pinned_scratch(void** out) {
     return H3DGS_OK;
 }
 
+// rows read as float4: rotations (preprocess_kernel, preprocess_backward_kernel) and shs when 3 M is a multiple of 4
+// (the SH kernels); a contiguous view at an odd float offset would be read misaligned
+static bool misaligned16(const void* p, const char* who) {
+    if ((((uintptr_t)p) & 15) == 0) return false;
+    set_error("%s must be 16-byte aligned (got %p)", who, p);
+    return true;
+}
+
+// the gradient rows the scatter reduces into as float4 (dL_drotations, and dL_dsh when 3 M is a multiple of 4)
+static bool grads_misaligned(const h3dgs_raster_args* a, const float* dL_dsh, const float* dL_drotations) {
+    return misaligned16(dL_drotations, "dL_drotations") ||
+           (((a->sh_coeffs * 3) & 3) == 0 && misaligned16(dL_dsh, "dL_dsh"));
+}
+
 static int check_args(const h3dgs_raster_args* a) {
     if (!a) { set_error("args is NULL"); return H3DGS_EINVAL; }
     if (a->P < 0 || a->image_width <= 0 || a->image_height <= 0) { set_error("bad sizes P=%d W=%d H=%d", a->P, a->image_width, a->image_height); return H3DGS_EINVAL; }
@@ -149,6 +163,8 @@ static int check_args(const h3dgs_raster_args* a) {
     if (a->bin_capacity > 0 && a->debug) { set_error("capacity mode has no host synchronisation: debug must be off"); return H3DGS_EINVAL; }
     if (!a->means3D && a->P > 0) { set_error("means3D is NULL"); return H3DGS_EINVAL; }
     if (!a->bg || !a->viewmatrix || !a->projmatrix || !a->campos) { set_error("bg/viewmatrix/projmatrix/campos must be device pointers"); return H3DGS_EINVAL; }
+    if (a->P > 0 && (misaligned16(a->rotations, "rotations") || (((a->sh_coeffs * 3) & 3) == 0 && misaligned16(a->shs, "shs"))))
+        return H3DGS_EINVAL;
     return H3DGS_OK;
 }
 
@@ -292,6 +308,7 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
         (a->scales && (!dL_dscales || !dL_drotations)) || (a->cov3D_precomp && !dL_dcov3D))) {
         set_error("backward: missing gradient output"); return H3DGS_EINVAL;
     }
+    if ((phases & 2) && grads_misaligned(a, dL_dsh, dL_drotations)) return H3DGS_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     const GeomLayout gl = geom_layout(a->P);
     const BinLayout bl = bin_layout(D);

@@ -36,7 +36,10 @@ def _f32c(t, name):
         raise RuntimeError(f"{name} must be a CUDA tensor")
     if t.dtype != torch.float32:
         t = t.float()
-    return t.contiguous()
+    t = t.contiguous()
+    # the kernels read rotations and SH rows as float4, and the library refuses rows that are not 16-byte aligned:
+    # a contiguous view at an odd float offset is copied (a fresh allocation is aligned)
+    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 def _i32c(t, name):

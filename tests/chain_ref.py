@@ -41,7 +41,7 @@ sum_x |d out / d x| e_x over the entries x of A and Sigma (computed by complex-s
 of each output to fp32.  Bounding it by magnitude chains instead would multiply the input errors by the condition
 factor (|a c| + b^2) / |denom| even where the true sensitivity is small (a needle's screen covariance is nearly rank one
 whatever the rounding of A), and would hide an fp32 evaluation of the block.
-Scattered rows add n U sum |contributions| for an n-term fp32 atomic sum in any order.
+Scattered rows add (n - 1) U sum |contributions| for an n-term fp32 atomic sum in any order (scatter_terms, scatter_tol).
 """
 import numpy as np
 
@@ -277,6 +277,33 @@ _DR_DQ = {
 }
 
 
+def scatter_terms(g, rows, v, e, a, acc, sign=None):
+    """The float64 statement of the scatter, one column: every full-size row r receives
+        sum_{i: c_i = r} t_i g_i  +  sum_{i: p_i = r, u_i != 0} u_i s_i g_i
+    over the rendered rows i in `rows` (the visible ones), with g_i = v (its error bound e and magnitude chain a, in
+    units of U, from chain_reference), u_i = fp32(1 - t_i) and the lerp taken only where u_i != 0 exactly (gather_fp32's
+    `lerp`, the kernels' decision), s_i the quaternion sign (rotations only, else None).  Accumulates into acc = (value,
+    error, magnitude, sum of |terms|, term count) [N] float64 arrays: each term carries its own error scaled by the
+    weight plus one rounding of the product w g."""
+    ref, err, mag, sm, cnt = acc
+    tw = g["t"][rows].astype(np.float64)
+    uw = g["u"][rows].astype(np.float64) * (sign if sign is not None else 1.0)
+    for idx, w, on in ((g["c"][rows], tw, np.ones(rows.size, bool)), (g["p"][rows], uw, g["lerp"][rows])):
+        idx, w, aw = idx[on], w[on], np.abs(w[on])
+        np.add.at(ref, idx, w * v[on])
+        np.add.at(err, idx, aw * e[on] + aw * np.abs(v[on]))
+        np.add.at(mag, idx, aw * a[on])
+        np.add.at(sm, idx, aw * np.abs(v[on]))
+        np.add.at(cnt, idx, 1)
+
+
+def scatter_tol(err, sm, cnt):
+    """budget of a full-size row from scatter_terms' sums: the terms' own errors and roundings, plus (n - 1) U sum |terms|
+    for the n-term fp32 atomic sum into the zero-filled row in an unspecified order (the first addition onto 0 is exact).
+    A row no visible row reaches, or reached by exact zeros only, has budget 0: it must hold exactly +0.0."""
+    return U * (err + np.maximum(cnt - 1, 0) * sm)
+
+
 def chain_reference(means3D, opacities, scales, rotations, shs, colors_precomp, cov3D_precomp, scale_modifier, view, proj,
                     campos, W, H, tanx, tany, sh_degree, radii, accum, sh_clamp, fclamp, fsign, do_depth,
                     ridx=None, pidx=None, ts=None, eps=1e-7):
@@ -433,19 +460,11 @@ def chain_reference(means3D, opacities, scales, rotations, shs, colors_precomp, 
                     for arr, x in ((ref, v), (err, e), (mag, a), (sm, np.abs(v)), (cnt, 1)):
                         arr[rows, col] += x
                     continue
-                tw = g["t"][rows].astype(np.float64)
-                uw = g["u"][rows].astype(np.float64) * (weight_u[rows] if weight_u is not None else 1.0)
-                for idx, w, on in ((g["c"][rows], tw, np.ones(rows.size, bool)), (g["p"][rows], uw, g["lerp"][rows])):
-                    idx, w, aw = idx[on], w[on], np.abs(w[on])
-                    np.add.at(ref[:, col], idx, w * v[on])
-                    # the product by the weight rounds once; the term's own error scales with |w|
-                    np.add.at(err[:, col], idx, aw * e[on] + aw * np.abs(v[on]))
-                    np.add.at(mag[:, col], idx, aw * a[on])
-                    np.add.at(sm[:, col], idx, aw * np.abs(v[on]))
-                    np.add.at(cnt[:, col], idx, 1)
+                scatter_terms(g, rows, v, e, a, (ref[:, col], err[:, col], mag[:, col], sm[:, col], cnt[:, col]),
+                              None if weight_u is None else weight_u[rows])
         # direct rows: a second part is one more fp32 add (dL/dmean3D of K8 + K9a, then += the SH term);
-        # scattered rows: an n-term fp32 atomic sum in any order
-        tol = U * (err + (cnt > 1) * sm) if not scatter else U * (err + cnt * sm)
+        # scattered rows: an n-term fp32 atomic sum in any order (scatter_tol)
+        tol = U * (err + (cnt > 1) * sm) if not scatter else scatter_tol(err, sm, cnt)
         out[name] = (ref, tol, mag)
 
     # dL/dmeans2D: one fp32 multiply of the sum by 0.5 W (0.5 H), so bit-exact; rows per rendered row

@@ -32,9 +32,9 @@ def _t(a, dtype=None):
     return torch.tensor(a, device="cuda", dtype=dtype if dtype is not None else (torch.int32 if a.dtype.kind == "i" else torch.float32))
 
 
-def run_backward(cam, sc, accum, deg, do_depth=False, mod=1.0, grad_rows=(0, 0), forward=None):
+def run_backward(cam, sc, accum, deg, do_depth=False, mod=1.0, grad_rows=(0, 0), forward=None, debug=False):
     """forward (or the given one) + the chain-rule phase on `accum` -> (gradients dict, radii, records, forward, K1's
-    view-space z)"""
+    view-space z); debug: the backward's serial path"""
     import torch
     from diff_gaussian_rasterization import _C
     from h3dgs import _lib
@@ -54,7 +54,7 @@ def run_backward(cam, sc, accum, deg, do_depth=False, mod=1.0, grad_rows=(0, 0),
     scratch = torch.zeros((_lib.lib().h3dgs_backward_scratch_bytes(P),), dtype=torch.uint8, device="cuda")
     scratch.view(torch.float32)[: P * 10] = f32(accum).reshape(-1)
     g = _C.rasterize_gaussians_backward(bg, m, radii, col, op, s, r, mod, cov, vm, pm, cam.tanfovx, cam.tanfovy, None, None,
-                                        sh, deg, cp, gb, n, bb, ib, False, ridx, pidx, ts, kids, do_depth, H, W, phases=2,
+                                        sh, deg, cp, gb, n, bb, ib, debug, ridx, pidx, ts, kids, do_depth, H, W, phases=2,
                                         scratch=scratch, grad_rows=grad_rows)
     names = ("means2D", "colors", "opacities", "means3D", "cov3D", "shs", "scales", "rotations")
     out = {k: v.cpu().numpy().copy() for k, v in zip(names, g) if v is not None and v.numel()}
@@ -62,25 +62,38 @@ def run_backward(cam, sc, accum, deg, do_depth=False, mod=1.0, grad_rows=(0, 0),
     return out, radii.cpu().numpy(), st["records"].cpu().numpy().copy(), forward, st["depths"].cpu().numpy().copy()
 
 
-def check_case(name, cam, sc, accum, deg=3, do_depth=False, mod=1.0, min_visible=0.5):
-    """run the case, compare every returned element with chain_ref; -> (report, radii, kbits, fclamp, K1 ratios)"""
-    got, radii, rec, fwd, depth = run_backward(cam, sc, accum, deg, do_depth, mod)
-    vis = radii > 0
-    assert vis.mean() >= min_visible, (name, vis.mean())
-    kb = rec[:, 7].view(np.uint32)
+def chain_ref_for(cam, sc, accum, deg, do_depth, mod, radii, kb):
+    """chain_ref's reference for one run, with the forward's decisions: radii, the SH clamp flags of kbits `kb` and the
+    frustum clamp as K1 evaluates it -> (ref dict, fclamp, tx/tz, ty/tz)"""
     scatter = sc.get("ridx") is not None
     means = (gather_fp32(sc["means3D"], sc.get("scales"), sc.get("rotations"), sc.get("shs"), sc["ridx"], sc["pidx"],
                          sc["ts"])["means3D"] if scatter else sc["means3D"])
     fcl, rx, ry = frustum_clamp_fp32(cam.world_view_transform, means, cam.tanfovx, cam.tanfovy)
-    # K1 evaluates the view transform in the order frustum_clamp_fp32 (and the backward) assume: its stored depth is the
-    # same fp32 value bit for bit, so a change of K1's order fails here as well as a change of the backward's
-    vz = view_xyz_fp32(cam.world_view_transform, means)[2]
-    assert np.array_equal(depth[vis].view(np.uint32), vz[vis].view(np.uint32)), name
     shc = np.stack([(kb >> (20 + ch)) & 1 for ch in range(3)], 1).astype(bool)
     ref = chain_reference(sc["means3D"], sc["opacities"], sc.get("scales"), sc.get("rotations"), sc.get("shs"),
                           sc.get("colors"), sc.get("cov3D"), mod, cam.world_view_transform, cam.full_proj_transform,
                           cam.camera_center, W, H, cam.tanfovx, cam.tanfovy, deg, radii, accum, shc, fcl,
                           np.stack([np.sign(rx), np.sign(ry)], 1), do_depth, sc.get("ridx"), sc.get("pidx"), sc.get("ts"))
+    return ref, fcl, rx, ry
+
+
+def check_case(name, cam, sc, accum, deg=3, do_depth=False, mod=1.0, min_visible=0.5, debug=False, keep=None):
+    """run the case, compare every returned element with chain_ref; -> (report, radii, kbits, fclamp, K1 ratios, got).
+    keep: a dict that receives the reference ('ref') and the forward ('forward')"""
+    got, radii, rec, fwd, depth = run_backward(cam, sc, accum, deg, do_depth, mod, debug=debug)
+    vis = radii > 0
+    assert vis.mean() >= min_visible, (name, vis.mean())
+    kb = rec[:, 7].view(np.uint32)
+    scatter = sc.get("ridx") is not None
+    ref, fcl, rx, ry = chain_ref_for(cam, sc, accum, deg, do_depth, mod, radii, kb)
+    means = (gather_fp32(sc["means3D"], sc.get("scales"), sc.get("rotations"), sc.get("shs"), sc["ridx"], sc["pidx"],
+                         sc["ts"])["means3D"] if scatter else sc["means3D"])
+    # K1 evaluates the view transform in the order frustum_clamp_fp32 (and the backward) assume: its stored depth is the
+    # same fp32 value bit for bit, so a change of K1's order fails here as well as a change of the backward's
+    vz = view_xyz_fp32(cam.world_view_transform, means)[2]
+    assert np.array_equal(depth[vis].view(np.uint32), vz[vis].view(np.uint32)), name
+    if keep is not None:
+        keep.update(ref=ref, forward=fwd)
     report = {}
     assert set(got) == set(ref), (name, sorted(got), sorted(ref))
     for k, (r, tol, _) in ref.items():
