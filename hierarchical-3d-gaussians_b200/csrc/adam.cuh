@@ -21,4 +21,26 @@ __device__ __forceinline__ void adam_element(float& param, float g, float& exp_a
     exp_avg_sq = v;
 }
 
+// one element of torch.optim.Adam's default CUDA path (_multi_tensor_adam, non-capturable; amsgrad off, weight_decay
+// 0), shared by train_single's exposure step (single_param.cu) and train_post's dense step (post_param.cu).  Its
+// foreach kernels compute in fp32 with FMA contraction:
+//   m = lerp(m, g, w) with w = (float)(1 - beta1): |w| < 0.5 ? fma(w, g - m, m) : fma(m - g, 1 - w, g)
+//   v = v * beta2;  v = fma((float)(1 - beta2), g * g, v)
+//   p = fma(step_size, m / (sqrt(v) / bc2_sqrt + eps), p)
+// with step_size = (float)(-(lr / (1 - beta1^t))) and bc2_sqrt = (float)sqrt(1 - beta2^t) formed in double (torch's
+// Python floats of the host step count t)
+__device__ __forceinline__ void torch_adam_element(float& param, float g, float& exp_avg, float& exp_avg_sq, float w,
+                                                   float beta2, float one_minus_b2, float step_size, float bc2_sqrt,
+                                                   float eps)
+{
+    const float m0 = exp_avg;
+    // at::native::lerp with opmath float, contracted
+    const float m = fabsf(w) < 0.5f ? __fmaf_rn(w, __fsub_rn(g, m0), m0) : __fmaf_rn(__fsub_rn(m0, g), __fsub_rn(1.f, w), g);
+    const float v = __fmaf_rn(one_minus_b2, __fmul_rn(g, g), __fmul_rn(exp_avg_sq, beta2));
+    const float den = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+    param = __fmaf_rn(step_size, __fdiv_rn(m, den), param);
+    exp_avg = m;
+    exp_avg_sq = v;
+}
+
 }  // namespace h3dgs

@@ -1,8 +1,9 @@
 // param_row.cuh -- the row-local pieces of a flat GaussianModel's parameter step, shared by train_coarse's
 // (coarse_param.cu) and train_single's (single_param.cu): the activations' backward from the rasterizer's activated
 // gradients to the six stored tensors, OurAdam on one row (adam.cuh), the big-Gaussian rescale and the activations the
-// next forward reads.  Every product, quotient and sum is rounded on its own (no FMA contraction); expf and logf are the
-// CUDA math library's accurate ones, as torch's exp / log / sigmoid use them.
+// next forward reads.  train_post's (post_param.cu) takes the quaternion norm and F.normalize's backward from here.
+// Every product, quotient and sum is rounded on its own (no FMA contraction); expf and logf are the CUDA math library's
+// accurate ones, as torch's exp / log / sigmoid use them.
 #pragma once
 #include "adam.cuh"
 
@@ -20,6 +21,22 @@ __device__ __forceinline__ void quat_norm(const float q[4], float& n, float& d)
     n = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q[0], q[0]), __fmul_rn(q[1], q[1])), __fmul_rn(q[2], q[2])),
                              __fmul_rn(q[3], q[3])));
     d = (n != n || n > 1e-12f) ? n : 1e-12f;
+}
+
+// F.normalize's backward: x / clamp_min(norm(x), 1e-12).  div: g / d to x, -g * ((x / d) / d) summed to d;
+// clamp_min passes where norm >= 1e-12; norm: x * (grad / norm), 0 where norm == 0.  g (the gradient of the normalized
+// quaternion) becomes the gradient of the stored one q
+__device__ __forceinline__ void normalize_backward(const float q[4], float g[4])
+{
+    float n, d;
+    quat_norm(q, n, d);
+    float gd = 0.f;
+#pragma unroll
+    for (int c = 0; c < 4; c++) gd = __fadd_rn(gd, __fmul_rn(-g[c], __fdiv_rn(__fdiv_rn(q[c], d), d)));
+    if (!(n >= 1e-12f)) gd = 0.f;
+    const float t = n == 0.f ? 0.f : __fdiv_rn(gd, n);
+#pragma unroll
+    for (int c = 0; c < 4; c++) g[c] = __fadd_rn(__fdiv_rn(g[c], d), __fmul_rn(q[c], t));
 }
 
 // with_rest = false leaves the f_rest part of shs to an element-parallel pass (its copy is the identity)
@@ -100,21 +117,12 @@ __device__ __forceinline__ void adam_row(const h3dgs_coarse_args& a, const Coars
         const size_t o = 3 * (size_t)i + c;
         adam_at(a, k, sc, 4, o, locked ? 0.f : __fmul_rn(a.grad_scales[o], a.scales[o]));
     }
-    // F.normalize's backward: x / clamp_min(norm(x), 1e-12).  div: g / d to x, -g * ((x / d) / d) summed to d;
-    // clamp_min passes where norm >= 1e-12; norm: x * (grad / norm), 0 where norm == 0
     float q[4], g[4];
 #pragma unroll
     for (int c = 0; c < 4; c++) { q[c] = a.params[5][4 * (size_t)i + c]; g[c] = a.grad_rotations[4 * (size_t)i + c]; }
-    float n, d;
-    quat_norm(q, n, d);
-    float gd = 0.f;
+    normalize_backward(q, g);
 #pragma unroll
-    for (int c = 0; c < 4; c++) gd = __fadd_rn(gd, __fmul_rn(-g[c], __fdiv_rn(__fdiv_rn(q[c], d), d)));
-    if (!(n >= 1e-12f)) gd = 0.f;
-    const float t = n == 0.f ? 0.f : __fdiv_rn(gd, n);
-#pragma unroll
-    for (int c = 0; c < 4; c++)
-        adam_at(a, k, sc, 5, 4 * (size_t)i + c, lock_all ? 0.f : __fadd_rn(__fdiv_rn(g[c], d), __fmul_rn(q[c], t)));
+    for (int c = 0; c < 4; c++) adam_at(a, k, sc, 5, 4 * (size_t)i + c, lock_all ? 0.f : g[c]);
 }
 
 __device__ __forceinline__ float stored_opacity_grad(const h3dgs_coarse_args& a, int i)

@@ -13,14 +13,9 @@
 //   rescale     rows >= scaffold_points, threshold float32(extent * 0.02) (:180-186);
 //   exposure    torch.optim.Adam([_exposure]) over the whole [n_images,3,4] tensor (:159-160): the frame's image row
 //               has its gradient, every other row a zero gradient, and all of them move as their moments decay.  Its
-//               arithmetic is that of torch's default CUDA path (_multi_tensor_adam, non-capturable), whose foreach
-//               kernels compute in fp32 with FMA contraction:
-//                 m = lerp(m, g, w) with w = (float)(1 - beta1): |w| < 0.5 ? fma(w, g - m, m) : fma(m - g, 1 - w, g)
-//                 v = v * beta2;  v = fma((float)(1 - beta2), g * g, v)
-//                 p = fma(step_size, m / (sqrt(v) / bc2_sqrt + eps), p)
-//               with step_size = (float)(-(lr / (1 - beta1^t))) and bc2_sqrt = (float)sqrt(1 - beta2^t) formed in double
-//               (torch's Python floats of the host step count t; torch.optim.Adam(capturable=True) would form them from
-//               a device fp32 step with fp32 pow instead).
+//               arithmetic is that of torch's default CUDA path (adam.cuh's torch_adam_element), with the bias
+//               corrections formed in double from the step count (torch's Python floats of the host step count;
+//               torch.optim.Adam(capturable=True) would form them from a device fp32 step with fp32 pow instead).
 // Launches: a one-thread prologue (step counts, bias corrections of both optimizers, the any-relevant word cleared),
 // the exposure Adam, for a full step the relevance pass, an element-parallel pass over f_rest and the row-local update
 // pass (train_coarse's, without f_rest); without the Gaussian step the update pass only rescales.
@@ -64,12 +59,9 @@ __global__ void __launch_bounds__(256) single_exposure_adam_kernel(h3dgs_single_
     if (e >= a.n_images * 12 || overflowed(a)) return;
     const SingleScratch& sc = *(const SingleScratch*)a.gauss.scratch;
     const float g = (e / 12 == *a.image_index) ? a.exposure_grad[e % 12] : 0.f;
-    const float m0 = a.exposure_exp_avg[e];
-    // at::native::lerp with opmath float, contracted
-    const float m = fabsf(x.w) < 0.5f ? __fmaf_rn(x.w, __fsub_rn(g, m0), m0) : __fmaf_rn(__fsub_rn(m0, g), __fsub_rn(1.f, x.w), g);
-    const float v = __fmaf_rn(x.omb2, __fmul_rn(g, g), __fmul_rn(a.exposure_exp_avg_sq[e], x.beta2));
-    const float den = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), sc.exp_bc2_sqrt), x.eps);
-    a.exposure[e] = __fmaf_rn(sc.exp_step_size, __fdiv_rn(m, den), a.exposure[e]);
+    float p = a.exposure[e], m = a.exposure_exp_avg[e], v = a.exposure_exp_avg_sq[e];
+    torch_adam_element(p, g, m, v, x.w, x.beta2, x.omb2, sc.exp_step_size, sc.exp_bc2_sqrt, x.eps);
+    a.exposure[e] = p;
     a.exposure_exp_avg[e] = m;
     a.exposure_exp_avg_sq[e] = v;
 }

@@ -29,6 +29,7 @@ EXPORTS = [
     "h3dgs_post_loss_forward", "h3dgs_post_loss_backward", "h3dgs_post_step_status",
     "h3dgs_post_loss_backward_exposure", "h3dgs_invdepth_l1_grad", "h3dgs_densify_stats", "h3dgs_single_step_status",
     "h3dgs_coarse_loss_forward", "h3dgs_coarse_loss_backward", "h3dgs_coarse_step_status", "h3dgs_coarse_param_step",
+    "h3dgs_post_param_step",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -84,6 +85,18 @@ class SingleArgs(C.Structure):
         ("lrs", C.c_void_p), ("exposure", C.c_void_p), ("exposure_exp_avg", C.c_void_p), ("exposure_exp_avg_sq", C.c_void_p),
         ("exposure_step", C.c_void_p), ("exposure_beta1", C.c_double), ("exposure_beta2", C.c_double),
         ("exposure_eps", C.c_double), ("exposure_grad", C.c_void_p), ("image_index", C.c_void_p), ("exposure_row", C.c_void_p),
+    ]
+
+
+POST_SCRATCH_BYTES = 64       # H3DGS_POST_SCRATCH_BYTES
+POST_STEP, POST_ACTIVATE, POST_BIAS = 0, 1, 2
+
+
+class PostArgs(C.Structure):
+    """struct h3dgs_post_args"""
+    _fields_ = [
+        ("gauss", CoarseArgs), ("lrs", C.c_void_p), ("locked", C.c_void_p), ("count", C.c_void_p),
+        ("extra_rows", C.c_int32), ("row_capacity", C.c_int32),
     ]
 
 
@@ -196,6 +209,9 @@ def bind(l):
     if hasattr(l, "h3dgs_single_param_step"):    # train_single's parameter step (likewise)
         l.h3dgs_single_param_step.restype = C.c_int
         l.h3dgs_single_param_step.argtypes = [C.POINTER(SingleArgs), C.c_int32, C.c_void_p]
+    if hasattr(l, "h3dgs_post_param_step"):      # train_post's parameter step (likewise)
+        l.h3dgs_post_param_step.restype = C.c_int
+        l.h3dgs_post_param_step.argtypes = [C.POINTER(PostArgs), C.c_int32, C.c_void_p]
     l.h3dgs_invdepth_l1_grad.restype = C.c_int
     l.h3dgs_invdepth_l1_grad.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
     l.h3dgs_densify_stats.restype = C.c_int

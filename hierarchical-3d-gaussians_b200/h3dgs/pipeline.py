@@ -187,16 +187,24 @@ def l1_step(scene, cam, bg, gt, threshold=None, sh_degree=3, fused=True, gt_read
     return loss, radii, n
 
 
-def post_step(scene, cam, bg, gt, threshold, lambda_dssim=0.2, exposure=None, mask=None, sh_degree=3):
+def post_step(scene, cam, bg, gt, threshold, lambda_dssim=0.2, exposure=None, mask=None, sh_degree=3, state=None,
+              update=True):
     """One step of train_post's loop body (train_post.py:91-142) on the exact path: render_hier_fused, then the objective
     (exposure, clamp, alpha mask, (1-l) L1 + l (1 - SSIM): h3dgs.loss.post_loss), then backward.  Gradients land in the
     scene's tensors.  Also the path that re-runs a frame h3dgs.poststep.GraphedPostStep flagged as overflowed.
+
+    state: a h3dgs.poststep.PostState (scene = state.make_scene()).  With update=True the iteration then ends with the
+    state's parameter step (train_post.py:167-192: the locks, the dense Adam step with state.set_learning_rate's xyz lr),
+    which also refreshes the scene's activated rows.  update=False leaves the state as it is (a saving iteration, whose
+    step follows scene.save, and the last iteration, which takes none).
     -> ((loss, l1, ssim) device scalars, radii, n cut rows)"""
     from .loss import post_loss
     scene.zero_grad()
     img, radii, n = render_hier_fused(scene, cam, bg, threshold, sh_degree)
     loss, l1, ssim = post_loss(img, gt, lambda_dssim, exposure, mask)
     loss.backward()
+    if state is not None and update:
+        state.param_step(scene)
     return (loss, l1, ssim), radii, n
 
 

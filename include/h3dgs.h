@@ -560,6 +560,41 @@ typedef struct h3dgs_single_args {
 } h3dgs_single_args;
 int h3dgs_single_param_step(const h3dgs_single_args* args, int32_t mode, void* stream);
 
+/* ---- train_post's parameter side (train_post.py:85, 165-192; csrc/post_param.cu) ----
+ * The model is GaussianModel.create_from_hier's: get_xyz identity, get_features = cat(f_dc, f_rest) with sh_coeffs
+ * coefficients, get_opacity = abs (NOT sigmoid), get_scaling = exp, get_rotation = F.normalize.  Its optimizer is
+ * torch.optim.Adam (training_setup(our_adam=False)), a DENSE step: every element of every row moves, rows outside the
+ * frame's cut with a zero gradient as their moments decay.
+ * gauss: the six stored tensors, their moments, the step count (one DEVICE int64 for the six groups), scratch
+ *   (H3DGS_POST_SCRATCH_BYTES), the activated rows (written) and their full-size gradients (read), as h3dgs_coarse_args;
+ *   gauss.lr[0] is unused (the xyz lr is *lrs, a DEVICE double the host fills each iteration: xyz_scheduler_args), the
+ *   other five are constants; gauss.skybox_points and gauss.rescale_threshold are unused (there is no rescale).
+ * locked: uint8 [N] (NULL = none): the rows whose six stored gradients are zeroed before the step -- the anchors
+ *   (anchors.bin) and, when skybox_locked, the last skybox_points rows (train_post.py:167-181).  A locked row is still
+ *   stepped, with g = 0.
+ * Overflow: a frame is skipped when gauss.scan_info (NULL = exact mode) has scan_info[2] set, or when count (h3dgs_lod_cut's
+ *   cut size, a DEVICE int32; NULL = exact mode) plus extra_rows (the skybox rows that follow the cut) exceeds
+ *   row_capacity.  A skipped frame changes no byte of state: parameters, moments, step count, activated rows.
+ * Per element, in the reference's order: the activation's backward (opacity: g * sign(o), sign(+-0) = 0; scaling:
+ *   g * exp(s) on the activated scale; rotation: F.normalize's backward on the row), the lock, torch.optim.Adam's default
+ *   CUDA arithmetic (adam.cuh's torch_adam_element; bias corrections of step + 1 formed in double on the device), then the
+ *   element's activation written into the activated row.
+ * mode H3DGS_POST_STEP: the step above, step += 1.
+ * mode H3DGS_POST_ACTIVATE: only the activations of every row (abs / exp / normalize / copy; grads, moments, step,
+ *   scratch and the overflow inputs unused).
+ * mode H3DGS_POST_BIAS: only the prologue: scratch receives float step_size[6] = (float)(-(lr / (1 - beta1^(step+1)))),
+ *   then float bc2_sqrt[6] = (float)sqrt(1 - beta2^(step+1)); the step count is unchanged. */
+#define H3DGS_POST_SCRATCH_BYTES 64
+enum { H3DGS_POST_STEP = 0, H3DGS_POST_ACTIVATE = 1, H3DGS_POST_BIAS = 2 };
+typedef struct h3dgs_post_args {
+    h3dgs_coarse_args gauss;
+    const double* lrs;
+    const uint8_t* locked;
+    const int32_t* count;
+    int32_t extra_rows, row_capacity;
+} h3dgs_post_args;
+int h3dgs_post_param_step(const h3dgs_post_args* args, int32_t mode, void* stream);
+
 /* ---- per-stage device timing (bench.py roofline) ----
  * When enabled, every stage launch is bracketed by two cudaEvents recorded on the stream
  * the kernel is launched on; h3dgs_profile_read synchronises them and returns the summed
