@@ -29,7 +29,7 @@ EXPORTS = [
     "h3dgs_post_loss_forward", "h3dgs_post_loss_backward", "h3dgs_post_step_status",
     "h3dgs_post_loss_backward_exposure", "h3dgs_invdepth_l1_grad", "h3dgs_densify_stats", "h3dgs_single_step_status",
     "h3dgs_coarse_loss_forward", "h3dgs_coarse_loss_backward", "h3dgs_coarse_step_status", "h3dgs_coarse_param_step",
-    "h3dgs_post_param_step",
+    "h3dgs_post_param_step", "h3dgs_densify_scratch_bytes", "h3dgs_densify",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
@@ -97,6 +97,21 @@ class PostArgs(C.Structure):
     _fields_ = [
         ("gauss", CoarseArgs), ("lrs", C.c_void_p), ("locked", C.c_void_p), ("count", C.c_void_p),
         ("extra_rows", C.c_int32), ("row_capacity", C.c_int32),
+    ]
+
+
+DENSIFY_COUNT, DENSIFY_WRITE, DENSIFY_RESET_OPACITY = 0, 1, 2
+
+
+class DensifyArgs(C.Structure):
+    """struct h3dgs_densify_args"""
+    _fields_ = [
+        ("N", C.c_int32), ("sh_coeffs", C.c_int32), ("scaffold_points", C.c_int32), ("skybox_points", C.c_int32),
+        ("max_grad", C.c_float), ("min_opacity", C.c_float), ("size_threshold", C.c_float),
+        ("params", C.c_void_p * 6), ("exp_avg", C.c_void_p * 6), ("exp_avg_sq", C.c_void_p * 6),
+        ("xyz_gradient_accum", C.c_void_p), ("max_radii2D", C.c_void_p), ("flags", C.c_void_p), ("scratch", C.c_void_p),
+        ("out_rows", C.c_int64), ("split_rows", C.c_int32), ("normals", C.c_void_p),
+        ("out_params", C.c_void_p * 6), ("out_exp_avg", C.c_void_p * 6), ("out_exp_avg_sq", C.c_void_p * 6),
     ]
 
 
@@ -212,6 +227,11 @@ def bind(l):
     if hasattr(l, "h3dgs_post_param_step"):      # train_post's parameter step (likewise)
         l.h3dgs_post_param_step.restype = C.c_int
         l.h3dgs_post_param_step.argtypes = [C.POINTER(PostArgs), C.c_int32, C.c_void_p]
+    if hasattr(l, "h3dgs_densify"):              # densify_and_prune / reset_opacity (likewise)
+        l.h3dgs_densify_scratch_bytes.restype = C.c_size_t
+        l.h3dgs_densify_scratch_bytes.argtypes = [C.c_int32]
+        l.h3dgs_densify.restype = C.c_int
+        l.h3dgs_densify.argtypes = [C.POINTER(DensifyArgs), C.c_int32, C.c_void_p]
     l.h3dgs_invdepth_l1_grad.restype = C.c_int
     l.h3dgs_invdepth_l1_grad.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
     l.h3dgs_densify_stats.restype = C.c_int

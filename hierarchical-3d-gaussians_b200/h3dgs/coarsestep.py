@@ -106,13 +106,21 @@ class CoarseState:
         return [dict(step=torch.tensor(step), exp_avg=m.clone(), exp_avg_sq=v.clone()) for m, v in zip(self.exp_avg, self.exp_avg_sq)]
 
     def copy_to_model(self, gaussians):
-        """the parameters, max_radii2D and the optimizer state into a GaussianModel (before scene.save or capture())"""
+        """the parameters, max_radii2D and the optimizer state into a GaussianModel (before scene.save or capture()).
+        When the row count differs from the model's (the state was densified on the device), each group gets a new
+        Parameter, bound in the optimizer group, its state and the model attribute, as densify_and_prune rebinds them"""
         opt = gaussians.optimizer
         groups = {g["name"]: g for g in opt.param_groups}
         with torch.no_grad():
             for a, n, p, s in zip(_MODEL_ATTRS, GROUPS, self.params, self.optimizer_state()):
                 t = getattr(gaussians, a)
-                t.data.copy_(p)
+                if t.shape == p.shape:
+                    t.data.copy_(p)
+                else:
+                    opt.state.pop(groups[n]["params"][0], None)
+                    t = torch.nn.Parameter(p.to(t.device, copy=True))
+                    groups[n]["params"][0] = t
+                    setattr(gaussians, a, t)
                 opt.state[groups[n]["params"][0]] = {k: (v.to(t.device) if k != "step" else v) for k, v in s.items()}
             gaussians.max_radii2D = self.max_radii2D.clone()
 

@@ -27,7 +27,8 @@ train_single.py:150-186 stay the caller's.  With a SingleState, graph B ends wit
 (the exposure's Adam, the skybox lock, the flattened relevance, OurAdam with this iteration's xyz lr, the rescale past
 the scaffold, the activations the next forward reads), the frame's exposure is the state's row of the image named by a
 device word, and the learning rates are device words: the whole iteration then replays without a host sync between
-two densifications.  densify_and_prune and reset_opacity stay torch on the GaussianModel (INTEGRATION.md).
+two densifications.  SingleState.densify_and_prune and reset_opacity (csrc/densify.cu) grow, shrink and reset the
+state itself, so the loop needs the GaussianModel only for saves and checkpoints (INTEGRATION.md).
 """
 import ctypes as C
 
@@ -55,12 +56,13 @@ class SingleState(CoarseState):
     densification statistics (stats: a pipeline.DensifyStats; state.max_radii2D is its max_radii2D).
 
     Device words the host fills without a sync: lrs = [xyz lr, exposure lr] (set_learning_rates, every iteration) and
-    image_index (set_image: the frame's row of the exposures).  exposure_grad [3,4] is the exact path's last dL/dE."""
+    image_index (set_image: the frame's row of the exposures).  exposure_grad [3,4] is the exact path's last dL/dE.
+    percent_dense (training_setup's, None until it is known) sets densify_and_prune's clone / split size threshold."""
 
     def __init__(self, params, skybox_points, lrs, exposure, betas=(0.9, 0.999), eps=1e-15, exp_avg=None, exp_avg_sq=None,
                  step=0, stats=None, skybox_locked=False, scaffold_points=None, scale_big_gauss=True, exposure_lr=0.0,
                  exposure_exp_avg=None, exposure_exp_avg_sq=None, exposure_step=0, exposure_betas=(0.9, 0.999),
-                 exposure_eps=1e-8):
+                 exposure_eps=1e-8, percent_dense=None):
         super().__init__(params, skybox_points, lrs, betas, eps, exp_avg, exp_avg_sq, step)
         dev, N = self.dev, self.N
         if stats is None:
@@ -85,6 +87,7 @@ class SingleState(CoarseState):
         self.image_index = torch.zeros(1, dtype=torch.int32, device=dev)
         self.exposure_grad = torch.zeros((3, 4), device=dev)
         self.scratch = torch.zeros(_lib.SINGLE_SCRATCH_BYTES, dtype=torch.uint8, device=dev)
+        self.percent_dense = None if percent_dense is None else float(percent_dense)
 
     # ---- per-iteration inputs (no host sync) ----------------------------------------------
     def set_learning_rates(self, xyz_lr, exposure_lr):
@@ -116,7 +119,8 @@ class SingleState(CoarseState):
         st = eo.state.get(gaussians._exposure, {})
         return cls(params, gaussians.skybox_points, lrs, gaussians._exposure, betas, eps, m, v, step, stats,
                    gaussians.skybox_locked, gaussians.scaffold_points, scale_big_gauss, g["lr"], st.get("exp_avg"),
-                   st.get("exp_avg_sq"), int(float(st["step"])) if "step" in st else 0, tuple(g["betas"]), g["eps"])
+                   st.get("exp_avg_sq"), int(float(st["step"])) if "step" in st else 0, tuple(g["betas"]), g["eps"],
+                   getattr(gaussians, "percent_dense", None))
 
     def copy_to_model(self, gaussians):
         """the parameters, both optimizers' state, the exposures and the statistics (xyz_gradient_accum and denom [N,1],
@@ -129,6 +133,80 @@ class SingleState(CoarseState):
                                                  exp_avg=self.exposure_exp_avg.clone(), exp_avg_sq=self.exposure_exp_avg_sq.clone())
             gaussians.xyz_gradient_accum = self.stats.xyz_gradient_accum.clone()
             gaussians.denom = self.stats.denom.clone()
+
+    # ---- densify_and_prune / reset_opacity (csrc/densify.cu) -------------------------------
+    def _densify_args(self):
+        a = _lib.DensifyArgs()
+        a.N, a.sh_coeffs, a.scaffold_points, a.skybox_points = self.N, self.sh_coeffs, self.scaffold_points, self.skybox_points
+        for k in range(6):
+            a.params[k], a.exp_avg[k], a.exp_avg_sq[k] = ptr(self.params[k]), ptr(self.exp_avg[k]), ptr(self.exp_avg_sq[k])
+        return a
+
+    def _launch_densify(self, args, mode):
+        with torch.cuda.device(self.dev):
+            _lib.check(_lib.lib().h3dgs_densify(C.byref(args), mode, torch.cuda.current_stream(self.dev).cuda_stream))
+
+    def densify_and_prune(self, max_grad, min_opacity, extent, generator=None, normals=None):
+        """GaussianModel.densify_and_prune(max_grad, min_opacity, extent) on the state -> the new row count N'.
+
+        Rows are decided from stats.xyz_gradient_accum and stats.max_radii2D and written once, in the reference's final
+        order [kept originals | clones | first split copies | second split copies]; new rows have zero moments, both
+        step counts and the exposures are kept, and the statistics restart at zero with N' rows (state.stats and
+        state.max_radii2D are new tensors: build the next step on them).  One host sync: the 16-byte count word, which
+        sizes the new tensors.  The split copies' standard normals z [2S,3] are drawn as
+        torch.empty((2S, 3)).normal_(generator=generator), the draw torch.normal(zeros, stds) makes before scaling, so
+        the default generator gives the reference's samples; normals= supplies them instead (tests).  max_grad must be
+        > 0 and min_opacity <= 0.15, as in train_single (0.0002 and 0.005): then no clone splits and no new row is
+        pruned, which the single-pass layout relies on."""
+        if self.percent_dense is None:
+            raise ValueError("percent_dense is unknown: build the state with from_model after training_setup, or pass it")
+        max_grad, min_opacity = float(np.float32(max_grad)), float(np.float32(min_opacity))
+        if not max_grad > 0.0 or not min_opacity <= float(np.float32(0.15)):
+            raise ValueError(f"densify_and_prune needs max_grad > 0 and min_opacity <= 0.15, not {max_grad}, {min_opacity}")
+        if generator is not None and normals is not None:
+            raise ValueError("pass either a generator or the normals, not both")
+        if generator is not None and torch.device(generator.device) != self.dev:
+            raise ValueError(f"the generator is on {generator.device}, the state on {self.dev}")
+        N, dev = self.N, self.dev
+        nbytes = int(_lib.lib().h3dgs_densify_scratch_bytes(N))
+        if nbytes == 0:
+            raise ValueError(f"{N} rows are too many to densify (3N must fit int32)")
+        flags = torch.empty(max(N, 1), dtype=torch.uint8, device=dev)
+        scratch = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+        off = (-scratch.data_ptr()) % 256
+        a = self._densify_args()
+        a.max_grad, a.min_opacity = max_grad, min_opacity
+        a.size_threshold = float(np.float32(self.percent_dense * float(extent)))
+        a.xyz_gradient_accum, a.max_radii2D = self.stats.xyz_gradient_accum.data_ptr(), self.stats.max_radii2D.data_ptr()
+        a.flags, a.scratch = flags.data_ptr(), scratch.data_ptr() + off
+        self._launch_densify(a, _lib.DENSIFY_COUNT)
+        K, Cn, S, N2 = (int(x) for x in scratch[off:off + 16].view(torch.int32).cpu())
+        if N2 < 0:
+            raise RuntimeError(f"densify_and_prune would make {K + Cn + 2 * S} rows, more than int32 indexes")
+        if normals is None:
+            normals = torch.empty((2 * S, 3), device=dev).normal_(generator=generator)
+        elif tuple(normals.shape) != (2 * S, 3) or normals.dtype != torch.float32 or normals.device != dev:
+            raise ValueError(f"normals must be float32 [{2 * S}, 3] on {dev}, not {normals.dtype} {tuple(normals.shape)} "
+                             f"on {normals.device}")
+        normals = normals.contiguous()
+        new = [torch.empty((N2,) + tuple(p.shape[1:]), device=dev) for p in self.params]
+        m = [torch.empty_like(p) for p in new]
+        v = [torch.empty_like(p) for p in new]
+        a.out_rows, a.split_rows, a.normals = N2, S, ptr(normals)
+        for k in range(6):
+            a.out_params[k], a.out_exp_avg[k], a.out_exp_avg_sq[k] = ptr(new[k]), ptr(m[k]), ptr(v[k])
+        self._launch_densify(a, _lib.DENSIFY_WRITE)
+        self.params, self.exp_avg, self.exp_avg_sq, self.N = new, m, v, N2
+        self.stats = DensifyStats(N2, dev)
+        self.max_radii2D = self.stats.max_radii2D
+        self.counts = dict(kept=K, cloned=Cn, split=S)
+        return N2
+
+    def reset_opacity(self):
+        """GaussianModel.reset_opacity in place: opacity = inverse_sigmoid(min(sigmoid(opacity), 0.01)) on the rows past
+        skybox_points, both opacity moments zero on every row; step counts and everything else unchanged.  The activated
+        rows are stale afterwards: make a new scene (make_scene) or activate the old one."""
+        self._launch_densify(self._densify_args(), _lib.DENSIFY_RESET_OPACITY)
 
     # ---- the parameter kernel --------------------------------------------------------------
     def _single_args(self, scene, cameras_extent=0.0, grads=None, exposure_grad=None, scan_info=None, exposure_row=None):

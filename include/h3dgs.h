@@ -560,6 +560,50 @@ typedef struct h3dgs_single_args {
 } h3dgs_single_args;
 int h3dgs_single_param_step(const h3dgs_single_args* args, int32_t mode, void* stream);
 
+/* ---- train_single's densify_and_prune and reset_opacity (scene/gaussian_model.py:510-514, 543-685; csrc/densify.cu) ----
+ * The six stored tensors params[g] and their OurAdam moments, in h3dgs_coarse_args' group order and shapes, N rows.
+ * mode H3DGS_DENSIFY_COUNT: per original row i, with g = xyz_gradient_accum[i] (NaN counts as 0), r = max_radii2D[i],
+ *   o = sigmoid(params[3][i]), p = powf(o, 0.2f), m = max(exp(params[4][i])) (NaN propagating), each op rounded on its own:
+ *     clone  (sqrt(g * g) * r) * p >= max_grad  and  o > 0.15f  and  m <= size_threshold (float32(percent_dense * extent))
+ *     split  (g * r) * p >= max_grad           and  o > 0.15f  and  m > size_threshold
+ *     keep   not split and not o < min_opacity
+ *   rows < scaffold_points are kept and never cloned or split.  flags[i] (uint8 [N]) = keep | clone << 1 | split << 2,
+ *   and the first 16 bytes of scratch receive the int32 count word {K kept, C clones, S splits, N' = K + C + 2S}, N' = -1
+ *   when it does not fit int32.  Needs max_grad > 0 (the clones' zero gradients never split) and min_opacity <= 0.15
+ *   (no clone or split copy is pruned).
+ * mode H3DGS_DENSIFY_WRITE (after COUNT, same flags and scratch): out_params / out_exp_avg / out_exp_avg_sq [N'] rows in
+ *   the reference's final order [kept originals in index order | clones | first copy of each split row | second copy]:
+ *   kept rows with their moments; clones a copy of the parameters; split copies k (first, normals row k) and S + k
+ *   (second) of the k-th split row: xyz + R(q) (z * exp(s) + 0) with R build_rotation's element-wise formula of the
+ *   stored q and the 3x3 product summed column by column, scaling log(exp(s) * (1.0f / 1.6f)), rotation, f_dc, f_rest
+ *   and opacity copied; every new row's moments 0.  normals: [2S][3] standard normals (NULL when S = 0).  out_rows and
+ *   split_rows are the host's copy of N' and S (checked: 0 <= 2 split_rows <= out_rows < 2^31).  The statistics are
+ *   not touched (densify_and_prune leaves them all zero at the new size).
+ * mode H3DGS_DENSIFY_RESET_OPACITY: params[3][i] = log(x / (1 - x)), x = min(sigmoid(params[3][i]), 0.01f) (NaN
+ *   propagating) for i >= skybox_points, in place; exp_avg[3] and exp_avg_sq[3] zero on every row.  Nothing else is read.
+ * No host synchronisation.  scratch: h3dgs_densify_scratch_bytes(N) device bytes, 256-byte aligned (0: N out of range,
+ * 3N must fit int32). */
+enum { H3DGS_DENSIFY_COUNT = 0, H3DGS_DENSIFY_WRITE = 1, H3DGS_DENSIFY_RESET_OPACITY = 2 };
+typedef struct h3dgs_densify_args {
+    int32_t N, sh_coeffs, scaffold_points, skybox_points;
+    float max_grad, min_opacity, size_threshold;
+    float* params[6];
+    float* exp_avg[6];
+    float* exp_avg_sq[6];
+    const float* xyz_gradient_accum;
+    const float* max_radii2D;
+    uint8_t* flags;
+    void* scratch;
+    int64_t out_rows;
+    int32_t split_rows;
+    const float* normals;
+    float* out_params[6];
+    float* out_exp_avg[6];
+    float* out_exp_avg_sq[6];
+} h3dgs_densify_args;
+size_t h3dgs_densify_scratch_bytes(int32_t N);
+int h3dgs_densify(const h3dgs_densify_args* args, int32_t mode, void* stream);
+
 /* ---- train_post's parameter side (train_post.py:85, 165-192; csrc/post_param.cu) ----
  * The model is GaussianModel.create_from_hier's: get_xyz identity, get_features = cat(f_dc, f_rest) with sh_coeffs
  * coefficients, get_opacity = abs (NOT sigmoid), get_scaling = exp, get_rotation = F.normalize.  Its optimizer is
