@@ -18,7 +18,7 @@ NO_FMAD = {"preprocess.cu", "binning.cu", "hierarchy.cu", "knn.cu", "hier_build.
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_forward.cu", "render_backward.cu",
            "preprocess_backward.cu", "hierarchy.cu", "loss.cu", "l1_loss.cu", "optim.cu", "peer.cu", "metrics.cu",
            "knn.cu", "hier_build.cu", "hier_merge.cu", "coarse_param.cu", "single_param.cu", "post_param.cu",
-           "densify.cu"]
+           "densify.cu", "lpips.cu"]
 
 
 def _needs_build(src, obj, deps):

@@ -12,14 +12,13 @@
 // The window weights travel as a kernel argument (no __constant__ upload, which would need a host synchronisation).
 #include <math.h>
 #include "common.cuh"
+#include "eval_pixel.cuh"
 
 namespace h3dgs {
 namespace {
 
 constexpr int kMR = 5, kMTS = 16, kMHalo = kMTS + 2 * kMR;      // 26
 struct Window { float w[11]; };
-
-__device__ __forceinline__ float clamp01(float v) { return fminf(fmaxf(v, 0.f), 1.f); }
 
 __device__ __forceinline__ double block_sum_256_d(double v, double* s_red) {
     v += __shfl_xor_sync(0xffffffffu, v, 16); v += __shfl_xor_sync(0xffffffffu, v, 8);
@@ -55,14 +54,8 @@ metrics_kernel(int H, int W, int x0, const float* __restrict__ img, const float*
         float a = 0.f, b = 0.f;                                     // zero padding at the crop border (conv2d padding=5)
         if (gy >= 0 && gy < H && gx >= 0 && gx < Wc) {
             const size_t p = (size_t)gy * W + x0 + gx;
-            if (exposure) {
-                // image.permute(1,2,0) @ E[:3,:3] + E[:3,3]: the matrix acts from the right, out[c] = sum_k img[k] E[k][c] + E[c][3]
-                a = img[p] * exposure[c] + img[plane + p] * exposure[4 + c] + img[2 * plane + p] * exposure[8 + c] + exposure[4 * c + 3];
-            } else {
-                a = img[(size_t)c * plane + p];
-            }
-            a = clamp01(a);
-            b = clamp01(gt[(size_t)c * plane + p]);
+            a = eval_value(img, exposure, plane, p, c);
+            b = eval_value(gt, nullptr, plane, p, c);
             if (out_img && ly >= kMR && ly < kMR + kMTS && lx >= kMR && lx < kMR + kMTS)
                 out_img[((size_t)c * H + gy) * Wc + gx] = a;        // exposed, clamped, cropped; before the mask
             if (mask) { const float m = mask[p]; a *= m; b *= m; }

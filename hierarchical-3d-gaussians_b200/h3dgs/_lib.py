@@ -30,10 +30,13 @@ EXPORTS = [
     "h3dgs_post_loss_backward_exposure", "h3dgs_invdepth_l1_grad", "h3dgs_densify_stats", "h3dgs_single_step_status",
     "h3dgs_coarse_loss_forward", "h3dgs_coarse_loss_backward", "h3dgs_coarse_step_status", "h3dgs_coarse_param_step",
     "h3dgs_post_param_step", "h3dgs_densify_scratch_bytes", "h3dgs_densify",
+    "h3dgs_lpips_weight_floats", "h3dgs_lpips_pack_weights", "h3dgs_lpips_scratch_floats", "h3dgs_lpips_features",
+    "h3dgs_lpips_distance", "h3dgs_lpips_conv",
 ]
 MAX_PEERS = 8
 IPC_HANDLE_BYTES = 64
 EVAL_ROW = 6            # H3DGS_EVAL_ROW: psnr, ssim, overflow, rows, D, longest tile list
+LPIPS_MIN_SIZE = 16     # H3DGS_LPIPS_MIN_SIZE
 
 
 class RasterArgs(C.Structure):
@@ -180,6 +183,20 @@ def bind(l):
         l.h3dgs_eval_metrics.restype = C.c_int
         l.h3dgs_eval_metrics.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] + [C.c_void_p] * 3 + \
             [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    if hasattr(l, "h3dgs_lpips_distance"):       # LPIPS (an emulation build has it when it compiles lpips.cu)
+        l.h3dgs_lpips_weight_floats.restype = C.c_int64
+        l.h3dgs_lpips_weight_floats.argtypes = []
+        l.h3dgs_lpips_pack_weights.restype = C.c_int
+        l.h3dgs_lpips_pack_weights.argtypes = [C.POINTER(C.c_void_p)] * 3 + [C.c_void_p]
+        l.h3dgs_lpips_scratch_floats.restype = C.c_int
+        l.h3dgs_lpips_scratch_floats.argtypes = [C.c_int32, C.c_int32] + [C.POINTER(C.c_int64)] * 3
+        l.h3dgs_lpips_features.restype = C.c_int
+        l.h3dgs_lpips_features.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4
+        l.h3dgs_lpips_distance.restype = C.c_int
+        l.h3dgs_lpips_distance.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 6 + \
+            [C.c_int32, C.c_void_p]
+        l.h3dgs_lpips_conv.restype = C.c_int
+        l.h3dgs_lpips_conv.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 4
     if hasattr(l, "h3dgs_dist_knn3"):            # 3-NN distances (an emulation build has it when it compiles knn.cu)
         l.h3dgs_knn_scratch_bytes.restype = C.c_size_t
         l.h3dgs_knn_scratch_bytes.argtypes = [C.c_int64]

@@ -1,4 +1,4 @@
-"""Sync-free evaluation of a hierarchy over a tau sweep: the numbers render_hierarchy.py reports (PSNR and SSIM over every
+"""Sync-free evaluation of a hierarchy over a tau sweep: the numbers render_hierarchy.py reports (PSNR, SSIM and, given a net, LPIPS over every
 test camera at tau in {0, 3, 6, 15}), with every frame replayed from one CUDA graph and one read-back at the end.
 
 The drop-in flow of render_hierarchy.py pays, per frame, two host round trips (the int of expand_to_size; num_rendered
@@ -11,10 +11,16 @@ clamps, crop, mask and the metric reductions with a syncing .double() each.  Her
     and the SSIM map sum in one pass, and a one-thread finisher that stores [psnr, ssim, status words] at a slot taken
     from a device counter.
 
+and, when an LpipsVGG net is given (lpips=),
+  * the image side of LPIPS (csrc/lpips.cu): the same exposed, clamped, cropped and masked image through VGG16 on TF32
+    tensor cores, compared with the target's taps; the value goes to the frame's slot of a device array.
+A second graph per camera size computes the target's taps; it is replayed once per camera, before that camera's taus,
+so a sweep of T taus runs T + 1 feature passes per camera where the reference runs 2T.
+
 Camera, target, mask, exposure and threshold are device-resident inputs copied in between replays.  A frame that does not
 fit the capacities (cut > row capacity, D > bin capacity, a tile list > sort capacity) is flagged in its row and re-run
-through the exact path (pipeline.render_hier_fused + the same metrics kernel) after the read-back.  LPIPS (VGG weights)
-and writing PNGs (torchvision) are not part of this module: keep_images returns the images instead.
+through the exact path (pipeline.render_hier_fused + the same metrics and LPIPS kernels) after the read-back.  Writing
+PNGs (torchvision) is not part of this module: keep_images returns the images instead.
 """
 import numpy as np
 import torch
@@ -40,11 +46,14 @@ class GraphedRender(GraphedLodCut):
     train_test_exp crop.  Inputs that change between replays: set_camera, set_threshold, and the static buffers
     `gt` [3,H,W], `exposure` [3,4], `mask` [H,W] (set_inputs copies into them).  Outputs: `image` (the raw rasterizer
     output, equal to pipeline.render_hier_fused's image whenever the frame fits), `out_image` [3,H,W-x0] when
-    keep_image (exposed, clamped, cropped), and one row per frame in `results` at slot `counter`++."""
+    keep_image (exposed, clamped, cropped), and one row per frame in `results` at slot `counter`++.
+
+    lpips: an LpipsVGG net, or None.  With one, target_features() computes the target's taps (a second graph, replayed
+    after set_inputs), and each frame also stores its LPIPS at the same slot of `lpips_values`."""
 
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None, bin_capacity=1 << 22,
                  sort_capacity=4096, exposure=False, mask=False, train_test_exp=False, keep_image=False, results=None,
-                 counter=None, max_frames=1024, capture=True):
+                 counter=None, max_frames=1024, capture=True, lpips=None, lpips_values=None):
         super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity)
         dev, H, W = self.dev, self.H, self.W
         self.image = self._zeros(3, H, W)
@@ -57,6 +66,12 @@ class GraphedRender(GraphedLodCut):
         self._warm_counter = torch.zeros(1, dtype=torch.int32, device=dev)          # the eager frame before capture
         self._warm_results = torch.zeros((1, _lib.EVAL_ROW), dtype=torch.float64, device=dev)
         self.args = self._raster_args(tanfovx, tanfovy)
+        self.lpips, self.graph_t = lpips, None
+        if lpips is not None:
+            lpips.scratch(H, W - self.x0)
+            self.lpips_values = lpips_values if lpips_values is not None else \
+                torch.zeros(self.results.shape[0], dtype=torch.float64, device=dev)
+            self._warm_lpips = torch.zeros(1, dtype=torch.float64, device=dev)
         if capture:
             self.capture()
 
@@ -70,10 +85,35 @@ class GraphedRender(GraphedLodCut):
         _metrics(self.L, self.H, self.W, self.image, self.gt, self.exposure, self.mask, self.x0, self.out_image, self.sums,
                  self.counter if counter is None else counter, self.results if results is None else results, self._stream(),
                  count=self.count, extra_rows=self.S, row_capacity=self.P, scan_info=self.scan_info())
+        if self.lpips is not None:
+            self.lpips.distance(self.image, self.lpips_values if results is None else self._warm_lpips, self.x0,
+                                self.exposure, self.mask, clamp=True, counter=self.counter if counter is None else counter,
+                                stream=self._stream())
+
+    def _target(self):
+        """the target's LPIPS taps (clamped, cropped, masked)"""
+        self.lpips.features(self.gt, self.x0, None, self.mask, clamp=True, stream=self._stream())
 
     def _warm_up(self):
         """capture()'s eager frame (sizes the state buffers): its row goes to a private slot"""
+        if self.lpips is not None:
+            self._target()
         self._part_a(self._warm_counter, self._warm_results)
+
+    def capture(self):
+        super().capture()
+        if self.lpips is not None:
+            self.graph_t = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph_t, pool=self.graph_a.pool()):
+                self._target()
+
+    def target_features(self):
+        """The target's taps from the current inputs, for the frames that follow: a graph replay (eager when not
+        captured).  Once per camera, after set_inputs."""
+        if self.graph_t is None:
+            self._target()
+        else:
+            self.graph_t.replay()
 
     def set_inputs(self, gt=None, mask=None, exposure=None):
         """Copy a frame's target [3,H,W], mask ([1,H,W] or [H,W]; None = ones) and exposure [3,4] (or larger: the top 3x4
@@ -104,7 +144,7 @@ class HierarchyEvaluator:
     the rows back once, re-runs the flagged frames through the exact path and averages."""
 
     def __init__(self, scene, cameras, targets, taus, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                 bg=None, sh_degree=3, capacities=None):
+                 bg=None, sh_degree=3, capacities=None, lpips=None):
         if not scene.hier:
             raise ValueError("evaluate_hierarchy needs a hierarchy scene")
         if len(targets) != len(cameras) or (masks is not None and len(masks) != len(cameras)) or \
@@ -119,7 +159,16 @@ class HierarchyEvaluator:
         self.masks = None if masks is None else [_stage(m) for m in masks]
         self.exposures = None if exposures is None else [None if e is None else e.to(dev).float() for e in exposures]
         self.n_frames = len(self.cameras) * len(self.taus)
-        self.results = torch.zeros((max(self.n_frames, 1), _lib.EVAL_ROW), dtype=torch.float64, device=dev)
+        self.lpips = lpips
+        n = max(self.n_frames, 1)
+        if lpips is None:
+            self.results = torch.zeros((n, _lib.EVAL_ROW), dtype=torch.float64, device=dev)
+            self.lpips_values = None
+        else:
+            # the rows, then one LPIPS value per frame: still one read-back for the sweep
+            self._readback = torch.zeros(n * (_lib.EVAL_ROW + 1), dtype=torch.float64, device=dev)
+            self.results = self._readback[:n * _lib.EVAL_ROW].view(n, _lib.EVAL_ROW)
+            self.lpips_values = self._readback[n * _lib.EVAL_ROW:]
         self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
         self.images = [[None] * len(self.cameras) for _ in self.taus] if keep_images else None
         groups = {}
@@ -139,7 +188,7 @@ class HierarchyEvaluator:
                              pipeline.fov_threshold(min(self.taus), cam), sh_degree=self.sh_degree,
                              exposure=self.exposures is not None, mask=self.masks is not None,
                              train_test_exp=self.train_test_exp, keep_image=self.keep_images, results=self.results,
-                             counter=self.counter, **kw)
+                             counter=self.counter, lpips=self.lpips, lpips_values=self.lpips_values, **kw)
 
     def _learn_capacities(self, cam):
         """Eager capacity-mode frames of the first view at the smallest and at the largest tau, with every row and a
@@ -183,6 +232,8 @@ class HierarchyEvaluator:
                 r.set_camera(cam)
                 r.set_inputs(self.targets[ci], None if self.masks is None else self.masks[ci],
                              None if self.exposures is None else self.exposures[ci])
+                if self.lpips is not None:
+                    r.target_features()
                 last = ci
             r.set_threshold(pipeline.fov_threshold(self.taus[ti], cam))
             r.frame()
@@ -191,7 +242,7 @@ class HierarchyEvaluator:
 
     def _exact(self, ti, ci):
         """One frame through the exact path (host-synchronising LOD cut and num_rendered sizing) and the same metrics
-        kernel -> its row (numpy)."""
+        kernel -> its row (numpy), and its LPIPS from the same kernels (None without a net)."""
         from diff_gaussian_rasterization import _C
         cam, r = self.cameras[ci], self._render_of(self.cameras[ci])
         thr = pipeline.fov_threshold(self.taus[ti], cam)
@@ -208,43 +259,64 @@ class HierarchyEvaluator:
             E = torch.eye(3, 4, device=self.dev) if self.exposures[ci] is None else self.exposures[ci][:3, :4].contiguous()
         _metrics(r.L, cam.H, cam.W, img.contiguous(), gt.float().contiguous(), E, mask, r.x0, out, r.sums, counter, results,
                  torch.cuda.current_stream(self.dev).cuda_stream, extra_rows=n + self.scene.skybox_points)
+        lp = None
+        if self.lpips is not None:
+            value = torch.zeros(1, dtype=torch.float64, device=self.dev)
+            self.lpips.features(gt.float().contiguous(), r.x0, None, mask, clamp=True)
+            self.lpips.distance(img.contiguous(), value, r.x0, E, mask, clamp=True, counter=counter)
+            lp = float(value.cpu()[0])
         row = results[0].cpu().numpy()
         row[4] = _C.last_num_rendered()
         if self.keep_images:
             self.images[ti][ci] = out
-        return row
+        return row, lp
 
     def finish(self):
         """-> dict(psnr={tau: mean}, ssim={tau: mean}, rows [n_taus, n_cameras, EVAL_ROW] (numpy; columns psnr, ssim,
         overflow, rows, D, longest tile list), rerun = frames re-run through the exact path, flagged = their
-        (tau index, camera index, capacity-mode row) -- what they needed --, images [tau][camera] when keep_images).
+        (tau index, camera index, capacity-mode row) -- what they needed --, images [tau][camera] when keep_images;
+        with an LPIPS net also lpips={tau: mean} and lpips_rows [n_taus, n_cameras]).
         The means are over the cameras, as render_hierarchy.py:111-119 averages them."""
-        flat = self.results[:self.n_frames].cpu().numpy()          # the one read-back of the sweep
+        if self.lpips is None:
+            flat = self.results[:self.n_frames].cpu().numpy()          # the one read-back of the sweep
+        else:
+            both = self._readback.cpu().numpy()
+            n = max(self.n_frames, 1)
+            flat, lp_flat = both[:n * _lib.EVAL_ROW].reshape(n, _lib.EVAL_ROW), both[n * _lib.EVAL_ROW:]
+            lp_rows = np.zeros((len(self.taus), len(self.cameras)))
         rows = np.zeros((len(self.taus), len(self.cameras), _lib.EVAL_ROW))
         for k, (ti, ci) in enumerate(self.order):
             rows[ti, ci] = flat[k]
+            if self.lpips is not None:
+                lp_rows[ti, ci] = lp_flat[k]
         flagged = []
         for ti in range(len(self.taus)):
             for ci in range(len(self.cameras)):
                 if rows[ti, ci, 2] != 0.0:
                     flagged.append((ti, ci, rows[ti, ci].copy()))
-                    rows[ti, ci] = self._exact(ti, ci)
+                    rows[ti, ci], lp = self._exact(ti, ci)
+                    if self.lpips is not None:
+                        lp_rows[ti, ci] = lp
         psnr = {t: float(rows[ti, :, 0].mean()) for ti, t in enumerate(self.taus)}
         ssim = {t: float(rows[ti, :, 1].mean()) for ti, t in enumerate(self.taus)}
-        return dict(psnr=psnr, ssim=ssim, rows=rows, rerun=len(flagged), flagged=flagged, images=self.images)
+        out = dict(psnr=psnr, ssim=ssim, rows=rows, rerun=len(flagged), flagged=flagged, images=self.images)
+        if self.lpips is not None:
+            out["lpips"] = {t: float(lp_rows[ti].mean()) for ti, t in enumerate(self.taus)}
+            out["lpips_rows"] = lp_rows
+        return out
 
 
 def evaluate_hierarchy(scene, cameras, targets, taus, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                       bg=None, sh_degree=3, capacities=None):
+                       bg=None, sh_degree=3, capacities=None, lpips=None):
     """The evaluation of render_hierarchy.py (render_set for every tau), sync-free.
 
     scene: pipeline.Scene with a hierarchy; cameras: pipeline.DeviceCamera per test view; targets: [3,H,W] per camera
     (device, or host: pinned here); masks: [1,H,W] alpha masks per camera (None entries = ones, the reference loader's
     fallback) or None; exposures: [3,4] per camera (None entries = no exposure for that camera, as render_post does for
     a missing one) or None; train_test_exp: evaluate the right half only; capacities: dict(row_capacity, bin_capacity,
-    sort_capacity) instead of the learned ones.  Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
+    sort_capacity) instead of the learned ones; lpips: an h3dgs.lpips.LpipsVGG net, to also report LPIPS.  Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
     -> see HierarchyEvaluator.finish."""
     ev = HierarchyEvaluator(scene, cameras, targets, taus, masks, exposures, train_test_exp, keep_images, bg, sh_degree,
-                            capacities)
+                            capacities, lpips)
     ev.enqueue()
     return ev.finish()

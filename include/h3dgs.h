@@ -362,6 +362,39 @@ int h3dgs_eval_metrics(int32_t H, int32_t W, const float* img, const float* gt, 
                        int32_t row_capacity, const uint32_t* scan_info, int32_t* counter, double* results,
                        int32_t max_rows, void* stream);
 
+/* ---- LPIPS of one frame pair, VGG16 (csrc/lpips.cu; lpipsPyTorch.lpips(x, y, 'vgg'), render_hierarchy.py:113) ----
+ * The network sees an H x Wc frame, Wc = W - x0, of a [3,H,W] frame: with clamp = 0 (lpips() itself) the frame's values
+ * as they are; with clamp != 0 (the evaluator, after h3dgs_eval_metrics) the value h3dgs_eval_metrics masks:
+ * exposure (NULL = none), clamp to [0,1], columns [x0, W), times mask [H,W] (NULL = none).  Then (v - mean) / std with
+ * mean (-.030, -.088, -.188), std (.458, .448, .450), and torchvision's vgg16().features up to index 29 on TF32 tensor
+ * cores with fp32 accumulation.  H and Wc must be >= H3DGS_LPIPS_MIN_SIZE (a smaller frame leaves a zero-size level).
+ *
+ * weights: h3dgs_lpips_weight_floats() device floats, packed once from host arrays by h3dgs_lpips_pack_weights:
+ *   conv_weight[13] [C_out][C_in][3][3] and conv_bias[13] [C_out] (features.{0,2,5,7,10,12,14,17,19,21,24,26,28}),
+ *   lin_weight[5] [C] (lin{k}.model.1.weight), all [host] fp32.
+ * Scratch sizes from h3dgs_lpips_scratch_floats(H, Wc): act (two activation buffers), taps (the five ReLU taps,
+ * NHWC [H_k][W_k][C_k] one after the other, H_k = H >> k', W_k = Wc >> k' with k' = 0, 1, 2, 3, 4), partials (doubles).
+ *
+ * h3dgs_lpips_features: the network on one frame, its taps stored in `taps` (the target side).
+ * h3dgs_lpips_distance: the network on the other frame against `taps`: per tap sum_c lin_c (n_x - n_y)^2 with
+ *   n = f / (sqrt(sum_c f^2) + 1e-10), its mean over the tap's pixels, the five means summed (in double, in a fixed
+ *   order: no atomics, the same bits on every run).  One device thread stores the value at out[slot], slot =
+ *   *counter - 1 (the slot h3dgs_eval_metrics just took) or 0 when counter is NULL; a slot >= max_rows is not stored.
+ * h3dgs_lpips_conv: one conv layer (0..12) + bias + ReLU, in [H][W][C_in] -> out [H][W][C_out] (layer 0: C_in = 8,
+ *   the three z-scored channels and five zeros).
+ * No host synchronisation; capturable. */
+#define H3DGS_LPIPS_MIN_SIZE 16
+int64_t h3dgs_lpips_weight_floats(void);
+int h3dgs_lpips_pack_weights(const float* const* conv_weight, const float* const* conv_bias, const float* const* lin_weight,
+                             float* packed);
+int h3dgs_lpips_scratch_floats(int32_t H, int32_t Wc, int64_t* act_floats, int64_t* tap_floats, int64_t* partial_doubles);
+int h3dgs_lpips_features(int32_t H, int32_t W, int32_t x0, const float* frame, const float* exposure, const float* mask,
+                         int32_t clamp, const float* weights, float* act, float* taps, void* stream);
+int h3dgs_lpips_distance(int32_t H, int32_t W, int32_t x0, const float* frame, const float* exposure, const float* mask,
+                         int32_t clamp, const float* weights, float* act, const float* taps, double* partials,
+                         const int32_t* counter, double* out, int32_t max_rows, void* stream);
+int h3dgs_lpips_conv(int32_t layer, int32_t H, int32_t W, const float* in, const float* weights, float* out, void* stream);
+
 /* ---- exact 3-nearest-neighbour distances (csrc/knn.cu; simple_knn._C.distCUDA2, scene/gaussian_model.py:21, 190-194) ----
  * points [P,3] float, mean_dist2 [P] float.  mean_dist2[i] = ((b0 + b1) + b2) / 3.0f, where b0 <= b1 <= b2 are the three
  * smallest d = (dx*dx + dy*dy) + dz*dz, dx = q.x - p.x (fp32, every operation rounded, no FMA), over the points q of OTHER
