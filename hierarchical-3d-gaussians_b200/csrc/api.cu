@@ -397,6 +397,7 @@ extern "C" int h3dgs_state_layout(int32_t P, int32_t W, int32_t H, int64_t D, co
     if (bin) {
         out->keys_sorted = (const uint64_t*)(bin + bl.keys_sorted);
         out->point_list = (const uint32_t*)(bin + bl.vals_sorted);
+        out->sorted_records = (const float*)(bin + bl.sorted_records);
     }
     if (img) {
         out->ranges = (const uint32_t*)(img + il.ranges);

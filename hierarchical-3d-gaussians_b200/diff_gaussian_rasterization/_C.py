@@ -231,4 +231,5 @@ def state_view(P, W, H, num_rendered, geomBuffer, binningBuffer, imageBuffer):
     if D > 0:
         out["keys_sorted"] = view(binningBuffer, v.keys_sorted, torch.int64, D)
         out["point_list"] = view(binningBuffer, v.point_list, torch.int32, D)
+        out["sorted_records"] = view(binningBuffer, v.sorted_records, torch.float32, D * 12).view(D, 12)
     return out

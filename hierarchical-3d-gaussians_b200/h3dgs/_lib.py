@@ -121,7 +121,8 @@ class DensifyArgs(C.Structure):
 class StateView(C.Structure):
     """struct h3dgs_state_view"""
     _fields_ = [(n, C.c_void_p) for n in ("depths", "tiles_touched", "point_offsets", "records", "keys_sorted",
-                                          "point_list", "ranges", "final_T", "n_contrib", "scan_info")]
+                                          "point_list", "ranges", "final_T", "n_contrib", "scan_info",
+                                          "sorted_records")]
 
 
 _lib = None

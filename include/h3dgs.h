@@ -191,6 +191,7 @@ typedef struct h3dgs_state_view {
     const float* final_T;             /* [H*W]                                                  */
     const uint32_t* n_contrib;        /* [H*W]                                                  */
     const uint32_t* scan_info;        /* [4] D, longest tile list, capacity overflow (0/1), prefiltered violated (0/1) */
+    const float* sorted_records;      /* [D][12] the records in tile-list order; word 7: kids (bits 0..15), block mask (16..31) */
 } h3dgs_state_view;
 int h3dgs_state_layout(int32_t P, int32_t W, int32_t H, int64_t num_rendered,
                        const void* geom_state, const void* binning_state, const void* image_state,

@@ -100,6 +100,7 @@ class Emu:
         if D > 0:
             out["point_list"] = view(b[1], v.point_list, np.uint32, D)
             out["keys_sorted"] = view(b[1], v.keys_sorted, np.uint64, D)
+            out["sorted_records"] = view(b[1], v.sorted_records, np.float32, 12 * D).reshape(D, 12)
         return out
 
     def backward(self, a, fwd, dL_dcolor, dL_dinvdepth=None, phases=3, scratch=None, outs=None):

@@ -1,6 +1,9 @@
 """CPU: csrc/reach_mask.cuh::block_mask16 (the 4x4-block reach mask the record gather stores and both blend kernels
-cull by), compiled for the host, against a brute-force per-pixel evaluation: 200 000 random projected Gaussians x tile
-positions -- no pixel with alpha >= 1/255 outside a marked block, and < 2 % of the marked blocks untouched."""
+cull by), compiled for the host, against a brute-force per-pixel evaluation in three families -- 200 000 random projected
+Gaussians x tile positions, needles (Gaussians seen edge-on, sigma_long 50 .. 600 px) over every tile they can reach, and
+opacities at prev / fp32 / next of 1/255 with means on pixel centres, tile corners and edges: no pixel with
+alpha >= 1/255 outside a marked block, and < 2 % of the marked blocks untouched, per family.  Conics that are not
+positive definite and non-finite means or conics get the fallback 0xFFFF, a NaN opacity 0."""
 import os
 import subprocess
 
