@@ -65,8 +65,8 @@ static void prof_drain() {
     g_prof_pending.clear();
 }
 
-// ---- side stream: zero-filling the full-size gradients (0.7 GB in scatter mode, pure DRAM
-// traffic) overlaps the issue-bound per-tile replay instead of preceding the chain rule ----
+// ---- side stream: zero-filling the smaller full-size gradients (scatter mode, pure DRAM traffic) beside the
+// issue-bound per-tile replay instead of before the chain rule ----
 struct SideStream { cudaStream_t s = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
 static SideStream g_side[64];
 static int side_stream(SideStream** out) {
@@ -322,10 +322,14 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
     bool zero_joined = true;
     SideStream* ss = nullptr;
     SideJoin side_guard;
-    // scatter mode: gradients have num_source rows and must start from zero.  The fill (0.7 GB on config #3) runs on the side
-    // stream beside the issue-bound replay; a caller that splits the phases asks for it with the replay (phases = 1 | 4) and
-    // tells the chain-rule call that it has happened (phases = 2 | 8) -- otherwise it would sit between the two, exposed
+    // scatter mode: gradients have num_source rows and must start from zero.  The fill (0.7 GB on config #3) goes with the
+    // issue-bound replay: dL/dSH (0.58 GB) in shares of the replay's own CTAs when the replay runs in this call (on the side
+    // stream it could not start before the replay, which holds every SM, had drained: render_backward.cu::zero_share), the
+    // other gradients on the side stream.  A caller that splits the phases asks for the fill with the replay (phases = 1 | 4)
+    // and tells the chain-rule call that it has happened (phases = 2 | 8) -- otherwise it would sit between the two, exposed
     const bool fill_now = a->render_indices && (((phases & 2) && !(phases & 8)) || (phases & 4));
+    const bool sh_fill_in_replay = fill_now && (phases & 1) && D > 0;
+    const size_t sh_floats = (size_t)a->num_source * a->sh_coeffs * 3;
     if (fill_now) {
         rc = side_stream(&ss);
         if (rc) return rc;
@@ -335,7 +339,7 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
         side_guard.arm(ss, s);
         H3_CUDA(cudaMemsetAsync(dL_dmeans3D, 0, N * 3 * sizeof(float), ss->s));
         H3_CUDA(cudaMemsetAsync(dL_dopacities, 0, N * sizeof(float), ss->s));
-        H3_CUDA(cudaMemsetAsync(dL_dsh, 0, N * (size_t)a->sh_coeffs * 3 * sizeof(float), ss->s));
+        if (!sh_fill_in_replay) H3_CUDA(cudaMemsetAsync(dL_dsh, 0, sh_floats * sizeof(float), ss->s));
         H3_CUDA(cudaMemsetAsync(dL_dscales, 0, N * 3 * sizeof(float), ss->s));
         H3_CUDA(cudaMemsetAsync(dL_drotations, 0, N * 4 * sizeof(float), ss->s));
         H3_CUDA(cudaEventRecord(ss->join, ss->s));
@@ -346,7 +350,7 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
         rc = launch_render_backward(b, (const uint32_t*)(img + il.ranges), (const Record*)(bin + bl.sorted_records),
                                     (const uint32_t*)(bin + bl.vals_sorted), (const float*)(img + il.final_T),
                                     (const uint32_t*)(img + il.n_contrib), (const uint32_t*)(img + il.tile_max_contrib),
-                                    dL_dcolor, dL_dinvdepth, accum, s);
+                                    dL_dcolor, dL_dinvdepth, accum, sh_fill_in_replay ? dL_dsh : nullptr, sh_floats, s);
         if (rc) return rc;
     }
     if ((phases & 1) && a->peer_count > 1) {
@@ -356,8 +360,8 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
     }
     if (!(phases & 2)) return H3DGS_OK;
     if (!zero_joined && !a->debug && !a->colors_precomp) {
-        // scatter mode: every output is an atomic reduction, so the SH kernel (side stream, right
-        // after its zero-fill) and the covariance kernel (main stream) run concurrently
+        // scatter mode: every output is an atomic reduction, so the SH kernel (side stream, after the
+        // fill) and the covariance kernel (main stream) run concurrently
         H3_CUDA(cudaEventRecord(ss->fork, s));                           // accum is complete at this point of s
         H3_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
         rc = launch_sh_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, dL_dmeans3D, dL_dsh, ss->s);

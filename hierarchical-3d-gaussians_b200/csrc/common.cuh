@@ -153,7 +153,8 @@ int launch_render_forward(const h3dgs_raster_args& a, const uint32_t* ranges, co
 int launch_render_backward(const h3dgs_raster_args& a, const uint32_t* ranges, const Record* sorted_records,
                            const uint32_t* point_list, const float* final_T, const uint32_t* n_contrib,
                            const uint32_t* tile_max_contrib, const float* dL_dcolor, const float* dL_dinvdepth,
-                           float* accum /*[P][10] zeroed*/, cudaStream_t s);
+                           float* accum /*[P][10] zeroed*/, float* zero /*zero_n floats to zero-fill, or NULL*/,
+                           size_t zero_n, cudaStream_t s);
 int launch_preprocess_backward(const h3dgs_raster_args& a, const int32_t* radii, const uint8_t* rank_mask, const Record* records,
                                const float* accum, float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh,
                                float* dL_dcolors, float* dL_dopacities, float* dL_dscales, float* dL_drots,

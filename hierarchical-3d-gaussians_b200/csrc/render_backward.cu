@@ -55,6 +55,24 @@ __device__ __forceinline__ int span_slot(int k) { const int q = k / (SPAN / 8); 
 
 constexpr int kBwdThreads = 128;      // two vertically adjacent pixels per thread (see render_forward.cu)
 
+// Scatter mode: the zero-fill of dL/dSH, the largest full-size gradient (0.58 GB on config #3), in shares of the replay's
+// CTAs.  A fill kernel on a side stream cannot run beside the replay, which holds every SM; it ran in the replay's tail and
+// after it, ahead of the chain rule.  Here it is a few dozen coalesced fire-and-forget stores per thread of an
+// issue-bound kernel.
+__device__ __forceinline__ void zero_share(float* p, size_t n)
+{
+    if (!p) return;
+    const size_t lead = (((16 - ((uintptr_t)p & 15)) & 15) / 4), head = lead < n ? lead : n;   // floats before the first float4
+    const size_t n4 = (n - head) / 4, tail = head + 4 * n4;
+    float4* body = reinterpret_cast<float4*>(p + head);
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n4; k += stride) body[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (blockIdx.x == 0 && threadIdx.x < 4) {
+        if (threadIdx.x < head) p[threadIdx.x] = 0.f;
+        if (tail + threadIdx.x < n) p[tail + threadIdx.x] = 0.f;
+    }
+}
+
 // Tile-sharded frames (NCCL or peer mode): the sums of a rank's own tiles go into ITS accumulator; the exchange follows
 // (peer mode: preprocess_backward.cu::peer_push_kernel stores the finished partial rows into the owners' staging areas).
 // A first version added every (tile, Gaussian) row straight into the owner's memory with system-scope red.add: 4-byte
@@ -66,13 +84,14 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
                        const float* __restrict__ bg, const float* __restrict__ final_T,
                        const uint32_t* __restrict__ n_contrib, const uint32_t* __restrict__ tile_max_contrib,
                        const float* __restrict__ dL_dcolor, const float* __restrict__ dL_dinvdepth,
-                       float* __restrict__ accum)
+                       float* __restrict__ accum, float* __restrict__ zero, size_t zero_n)
 {
     __shared__ __align__(128) Record s_rec[kBwdStages][kBwdBatch];
     __shared__ uint32_t s_id[kBwdStages][kBwdBatch];
     __shared__ __align__(8) uint64_t s_full[kBwdStages];
     __shared__ __align__(16) uint8_t s_list[GROUPS ? kBwdThreads / 32 : 1][4][GROUPS ? kBwdBatch : 4];   // group walk: per warp, four lists of entry positions
 
+    zero_share(zero, zero_n);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile_x = blockIdx.x % gx;
     const int tile_y = (blockIdx.x / gx) * shard_count + shard_index;
@@ -256,13 +275,16 @@ render_backward_kernel(int W, int H, int gx, int shard_count, int shard_index, c
 int launch_render_backward(const h3dgs_raster_args& a, const uint32_t* ranges, const Record* sorted_records,
                            const uint32_t* point_list, const float* final_T, const uint32_t* n_contrib,
                            const uint32_t* tile_max_contrib, const float* dL_dcolor, const float* dL_dinvdepth,
-                           float* accum, cudaStream_t s)
+                           float* accum, float* zero, size_t zero_n, cudaStream_t s)
 {
     const int W = a.image_width, H = a.image_height;
     const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
     const int sc = a.shard_count > 0 ? a.shard_count : 1, si = a.shard_count > 0 ? a.shard_index : 0;
     const int rows = (gy + sc - 1 - si) / sc;
-    if (rows <= 0 || gx <= 0) return H3DGS_OK;
+    if (rows <= 0 || gx <= 0) {                      // no tile of ours: the fill still happens
+        if (zero) H3_CUDA(cudaMemsetAsync(zero, 0, zero_n * sizeof(float), s));
+        return H3DGS_OK;
+    }
     const bool hier = a.interpolation_weights != nullptr;
     const bool depth = a.do_depth != 0 && dL_dinvdepth != nullptr;
     const dim3 grid(gx * rows), block(kBwdThreads);
@@ -271,7 +293,7 @@ int launch_render_backward(const h3dgs_raster_args& a, const uint32_t* ranges, c
 #define LAUNCH(HI, DE, GR)                                                                                          \
     render_backward_kernel<HI, DE, GR><<<grid, block, 0, s>>>(W, H, gx, sc, si, (const uint2*)ranges, sorted_records, \
                                                               point_list, a.bg, final_T, n_contrib, tile_max_contrib, \
-                                                              dL_dcolor, dL_dinvdepth, accum)
+                                                              dL_dcolor, dL_dinvdepth, accum, zero, zero_n)
 #define LAUNCH2(HI, DE) do { if (groups) LAUNCH(HI, DE, true); else LAUNCH(HI, DE, false); } while (0)
     if (hier) { if (depth) LAUNCH2(true, true); else LAUNCH2(true, false); }
     else      { if (depth) LAUNCH2(false, true); else LAUNCH2(false, false); }
