@@ -7,8 +7,8 @@
 // target while its parent is not, or when it is too coarse but holds leaf Gaussians),
 // with an order-preserving compaction -- one kernel, one pass (lod_cut_fused_kernel).
 // HBM-bound: 28 B node + 32 B box (+ the parent's box, an L2 hit in BFS order) per node.
-#include <float.h>
 #include "common.cuh"
+#include "lod_size.cuh"
 #include "tma.cuh"
 
 namespace h3dgs {
@@ -16,14 +16,7 @@ namespace h3dgs {
 struct Node { int depth, parent, start, count_leafs, count_merged, start_children, count_children; };
 
 __device__ __forceinline__ float node_size(const float4* __restrict__ boxes, int id, float vx, float vy, float vz) {
-    const float4 mn = __ldg(boxes + 2 * (size_t)id), mx = __ldg(boxes + 2 * (size_t)id + 1);
-    const bool inside = vx >= mn.x && vx <= mx.x && vy >= mn.y && vy <= mx.y && vz >= mn.z && vz <= mx.z;
-    if (inside) return FLT_MAX;
-    const float cx = fmaxf(mn.x, fminf(mx.x, vx)) - vx;
-    const float cy = fmaxf(mn.y, fminf(mx.y, vy)) - vy;
-    const float cz = fmaxf(mn.z, fminf(mx.z, vz)) - vz;
-    const float dist = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), __fmul_rn(cz, cz)));
-    return mn.w / dist;
+    return box_size(__ldg(boxes + 2 * (size_t)id), __ldg(boxes + 2 * (size_t)id + 1), vx, vy, vz);
 }
 
 // transition weight of node `id` under `parent` (oracle_interpolation_weights)
@@ -72,16 +65,6 @@ interpolation_weights_kernel(int n, const int* __restrict__ node_indices, float 
 constexpr int kCutThreads = 256, kCutItems = 4, kCutTile = kCutThreads * kCutItems;
 constexpr unsigned long long kTileAgg = 1ull << 62, kTilePrefix = 2ull << 62, kTileValue = (1ull << 62) - 1;
 constexpr size_t kCutSmem = (size_t)kCutTile * 7 * sizeof(int) + (size_t)kCutTile * 2 * sizeof(float4);
-
-__device__ __forceinline__ float box_size(const float4 mn, const float4 mx, float vx, float vy, float vz) {
-    const bool inside = vx >= mn.x && vx <= mx.x && vy >= mn.y && vy <= mx.y && vz >= mn.z && vz <= mx.z;
-    if (inside) return FLT_MAX;
-    const float cx = fmaxf(mn.x, fminf(mx.x, vx)) - vx;
-    const float cy = fmaxf(mn.y, fminf(mx.y, vy)) - vy;
-    const float cz = fmaxf(mn.z, fminf(mx.z, vz)) - vz;
-    const float dist = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), __fmul_rn(cz, cz)));
-    return mn.w / dist;
-}
 
 __global__ void __launch_bounds__(kCutThreads, 3)
 lod_cut_fused_kernel(int N, const int* __restrict__ nodes, const float4* __restrict__ boxes, float target,

@@ -1,0 +1,20 @@
+// lod_size.cuh -- the size of a hierarchy node's box seen from the viewpoint, the one quantity the LOD cut
+// (hierarchy.cu) and the budget's threshold selection (lod_budget.cu) compare against a threshold.  Both files are
+// compiled with -fmad=false, so this expression rounds the same way in each, operation by operation.
+#pragma once
+#include <float.h>
+
+namespace h3dgs {
+
+// min.w / distance from the viewpoint to the box, FLT_MAX when the viewpoint is inside (faces included)
+__device__ __forceinline__ float box_size(const float4 mn, const float4 mx, float vx, float vy, float vz) {
+    const bool inside = vx >= mn.x && vx <= mx.x && vy >= mn.y && vy <= mx.y && vz >= mn.z && vz <= mx.z;
+    if (inside) return FLT_MAX;
+    const float cx = fmaxf(mn.x, fminf(mx.x, vx)) - vx;
+    const float cy = fmaxf(mn.y, fminf(mx.y, vy)) - vy;
+    const float cz = fmaxf(mn.z, fminf(mx.z, vz)) - vz;
+    const float dist = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), __fmul_rn(cz, cz)));
+    return mn.w / dist;
+}
+
+}  // namespace h3dgs

@@ -18,7 +18,7 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 EXPORTS = [
     "h3dgs_rasterize_forward", "h3dgs_rasterize_backward", "h3dgs_backward_scratch_bytes", "h3dgs_mark_visible",
     "h3dgs_state_layout", "h3dgs_expand_to_size", "h3dgs_expand_scratch_bytes", "h3dgs_get_interpolation_weights",
-    "h3dgs_lod_cut",
+    "h3dgs_lod_cut", "h3dgs_lod_budget", "h3dgs_lod_budget_scratch_bytes",
     "h3dgs_last_error", "h3dgs_version", "h3dgs_launch_count",
     "h3dgs_profile_enable", "h3dgs_profile_reset", "h3dgs_profile_read", "h3dgs_stage_name",
     "h3dgs_l1_ssim_forward", "h3dgs_l1_ssim_backward", "h3dgs_l1_loss_grad", "h3dgs_l1_loss_grad_peer", "h3dgs_step_status", "h3dgs_sparse_adam",
@@ -180,6 +180,11 @@ def bind(l):
         l.h3dgs_peer_barrier_status.argtypes = [C.c_void_p, C.c_void_p]
     l.h3dgs_lod_cut.restype = C.c_int
     l.h3dgs_lod_cut.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_float] + [C.c_void_p] * 10
+    if hasattr(l, "h3dgs_lod_budget"):           # LOD budget (an emulation build has it when it compiles lod_budget.cu)
+        l.h3dgs_lod_budget_scratch_bytes.restype = C.c_size_t
+        l.h3dgs_lod_budget_scratch_bytes.argtypes = [C.c_int32]
+        l.h3dgs_lod_budget.restype = C.c_int
+        l.h3dgs_lod_budget.argtypes = [C.c_int32] + [C.c_void_p] * 3 + [C.c_float, C.c_void_p, C.c_int32] + [C.c_void_p] * 5
     if hasattr(l, "h3dgs_eval_metrics"):         # evaluation metrics (an emulation build has it when it compiles metrics.cu)
         l.h3dgs_eval_metrics.restype = C.c_int
         l.h3dgs_eval_metrics.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] + [C.c_void_p] * 3 + \
@@ -291,7 +296,7 @@ def launch_count():
     return int(lib().h3dgs_launch_count())
 
 
-STAGES = 16
+STAGES = 17
 
 
 def profile_enable(on=True):

@@ -49,12 +49,17 @@ class GraphedRender(GraphedLodCut):
     keep_image (exposed, clamped, cropped), and one row per frame in `results` at slot `counter`++.
 
     lpips: an LpipsVGG net, or None.  With one, target_features() computes the target's taps (a second graph, replayed
-    after set_inputs), and each frame also stores its LPIPS at the same slot of `lpips_values`."""
+    after set_inputs), and each frame also stores its LPIPS at the same slot of `lpips_values`.
+
+    budget: a Gaussian budget (GraphedLodCut): the cut's threshold is then chosen on the device, no finer than the
+    threshold (the floor; set_threshold), and each frame also stores [threshold, rows, unmet] at its slot of
+    `budget_values`."""
 
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None, bin_capacity=1 << 22,
                  sort_capacity=4096, exposure=False, mask=False, train_test_exp=False, keep_image=False, results=None,
-                 counter=None, max_frames=1024, capture=True, lpips=None, lpips_values=None):
-        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity)
+                 counter=None, max_frames=1024, capture=True, lpips=None, lpips_values=None, budget=None,
+                 budget_values=None):
+        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget)
         dev, H, W = self.dev, self.H, self.W
         self.image = self._zeros(3, H, W)
         self._init_inputs(exposure, mask)
@@ -72,6 +77,10 @@ class GraphedRender(GraphedLodCut):
             self.lpips_values = lpips_values if lpips_values is not None else \
                 torch.zeros(self.results.shape[0], dtype=torch.float64, device=dev)
             self._warm_lpips = torch.zeros(1, dtype=torch.float64, device=dev)
+        if budget is not None:
+            self.budget_values = budget_values if budget_values is not None else \
+                torch.zeros((self.results.shape[0], 3), dtype=torch.float64, device=dev)
+            self._warm_budget = torch.zeros((1, 3), dtype=torch.float64, device=dev)
         if capture:
             self.capture()
 
@@ -81,6 +90,10 @@ class GraphedRender(GraphedLodCut):
     def _part_a(self, counter=None, results=None):
         """LOD cut -> forward -> metrics pass, whose row goes to slot counter++ of results"""
         self._cut()
+        if self.budget_dev is not None:
+            rec = torch.cat((self.threshold_dev.double(), self.budget_info[:2].double())).unsqueeze(0)
+            (self.budget_values if results is None else self._warm_budget).index_copy_(
+                0, (self.counter if counter is None else counter).long(), rec)
         self._forward(self.image)
         _metrics(self.L, self.H, self.W, self.image, self.gt, self.exposure, self.mask, self.x0, self.out_image, self.sums,
                  self.counter if counter is None else counter, self.results if results is None else results, self._stream(),
@@ -141,16 +154,28 @@ def _stage(t):
 class HierarchyEvaluator:
     """evaluate_hierarchy in three steps: __init__ learns the capacities and captures one GraphedRender per camera size
     (host synchronisations happen here), enqueue() runs the whole sweep without synchronising the host, finish() reads
-    the rows back once, re-runs the flagged frames through the exact path and averages."""
+    the rows back once, re-runs the flagged frames through the exact path and averages.
+
+    With budgets (and taus None) the sweep runs over Gaussian budgets instead of taus: each frame's threshold is the finest
+    one, no finer than fov_threshold(tau_floor, camera), whose cut holds at most the budget's rows (GraphedRender's
+    budget=), and the frame's [threshold, rows, unmet] travel in the same read-back."""
 
     def __init__(self, scene, cameras, targets, taus, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                 bg=None, sh_degree=3, capacities=None, lpips=None):
+                 bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0):
         if not scene.hier:
             raise ValueError("evaluate_hierarchy needs a hierarchy scene")
+        if (taus is None) == (budgets is None):
+            raise ValueError("give taus or budgets (with tau_floor), not both")
+        if budgets is not None and min(budgets, default=0) < 0:
+            raise ValueError("budgets must be >= 0")
         if len(targets) != len(cameras) or (masks is not None and len(masks) != len(cameras)) or \
                 (exposures is not None and len(exposures) != len(cameras)):
             raise ValueError("targets, masks and exposures need one entry per camera")
-        self.scene, self.cameras, self.taus = scene, list(cameras), [float(t) for t in taus]
+        self.scene, self.cameras = scene, list(cameras)
+        self.taus = None if taus is None else [float(t) for t in taus]
+        self.budgets = None if budgets is None else [int(b) for b in budgets]
+        self.tau_floor = float(tau_floor)
+        self.sweep = self.taus if budgets is None else self.budgets       # what a frame's first index runs over
         self.sh_degree, self.train_test_exp, self.keep_images = int(sh_degree), bool(train_test_exp), bool(keep_images)
         dev = scene.means3D.device
         self.dev = dev
@@ -158,37 +183,41 @@ class HierarchyEvaluator:
         self.targets = [_stage(t) for t in targets]
         self.masks = None if masks is None else [_stage(m) for m in masks]
         self.exposures = None if exposures is None else [None if e is None else e.to(dev).float() for e in exposures]
-        self.n_frames = len(self.cameras) * len(self.taus)
+        self.n_frames = len(self.cameras) * len(self.sweep)
         self.lpips = lpips
         n = max(self.n_frames, 1)
-        if lpips is None:
-            self.results = torch.zeros((n, _lib.EVAL_ROW), dtype=torch.float64, device=dev)
-            self.lpips_values = None
-        else:
-            # the rows, then one LPIPS value per frame: still one read-back for the sweep
-            self._readback = torch.zeros(n * (_lib.EVAL_ROW + 1), dtype=torch.float64, device=dev)
-            self.results = self._readback[:n * _lib.EVAL_ROW].view(n, _lib.EVAL_ROW)
-            self.lpips_values = self._readback[n * _lib.EVAL_ROW:]
+        # the rows, then one LPIPS value per frame, then [threshold, rows, unmet] per frame of a budget sweep: one
+        # read-back for the sweep
+        widths = [_lib.EVAL_ROW, 1 if lpips is not None else 0, 3 if budgets is not None else 0]
+        self._readback = torch.zeros(n * sum(widths), dtype=torch.float64, device=dev)
+        self.results = self._readback[:n * widths[0]].view(n, widths[0])
+        self.lpips_values = self._readback[n * widths[0]:n * (widths[0] + widths[1])] if lpips is not None else None
+        self.budget_values = self._readback[n * (widths[0] + widths[1]):].view(n, 3) if budgets is not None else None
         self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.images = [[None] * len(self.cameras) for _ in self.taus] if keep_images else None
+        self.images = [[None] * len(self.cameras) for _ in self.sweep] if keep_images else None
         groups = {}
         for ci, cam in enumerate(self.cameras):
             groups.setdefault((cam.W, cam.H, float(cam.tanfovx), float(cam.tanfovy)), []).append(ci)
-        self.order = []                                  # (tau index, camera index) in slot order
+        self.order = []                                  # (tau or budget index, camera index) in slot order
         self.renders = {}
         for key, cis in groups.items():
             caps = capacities or self._learn_capacities(self.cameras[cis[0]])
             self.renders[key] = self._make(self.cameras[cis[0]], capture=True, **caps)
             for ci in cis:
-                self.order += [(ti, ci) for ti in range(len(self.taus))]
+                self.order += [(ti, ci) for ti in range(len(self.sweep))]
         self.frame_of = {k: i for i, k in enumerate(self.order)}
 
+    def _floor(self, cam):
+        """the finest threshold of the sweep: the smallest tau's, or the floor of a budget sweep"""
+        return pipeline.fov_threshold(self.tau_floor if self.taus is None else min(self.taus), cam)
+
     def _make(self, cam, **kw):
-        return GraphedRender(self.scene, cam.W, cam.H, cam.tanfovx, cam.tanfovy, self.bg,
-                             pipeline.fov_threshold(min(self.taus), cam), sh_degree=self.sh_degree,
-                             exposure=self.exposures is not None, mask=self.masks is not None,
+        budget = None if self.budgets is None else max(self.budgets)
+        return GraphedRender(self.scene, cam.W, cam.H, cam.tanfovx, cam.tanfovy, self.bg, self._floor(cam),
+                             sh_degree=self.sh_degree, exposure=self.exposures is not None, mask=self.masks is not None,
                              train_test_exp=self.train_test_exp, keep_image=self.keep_images, results=self.results,
-                             counter=self.counter, lpips=self.lpips, lpips_values=self.lpips_values, **kw)
+                             counter=self.counter, lpips=self.lpips, lpips_values=self.lpips_values, budget=budget,
+                             budget_values=self.budget_values, **kw)
 
     def _learn_capacities(self, cam):
         """Eager capacity-mode frames of the first view at the smallest and at the largest tau, with every row and a
@@ -196,15 +225,20 @@ class HierarchyEvaluator:
         not fit (then once more with room for D).  Both ends are needed: the finest cut has the most rows, but the
         coarsest has the largest Gaussians and so the most (tile, Gaussian) entries.  Other views may need more than the
         first: capacities = rows x 1.25, D x 1.5 and the next power of two above twice the longest list; a frame that
-        still does not fit is re-run exactly."""
+        still does not fit is re-run exactly.  A budget sweep probes its smallest and largest budget at the floor; its
+        rows are bounded by the largest budget (plus the skybox rows) instead."""
         N = self.scene.means3D.shape[0]
         rows = D = longest = 0
-        for tau in sorted({min(self.taus), max(self.taus)}):
+        if self.taus is None:
+            ends = [(self._floor(cam), b) for b in sorted({min(self.budgets), max(self.budgets)})]
+        else:
+            ends = [(pipeline.fov_threshold(tau, cam), None) for tau in sorted({min(self.taus), max(self.taus)})]
+        for thr, budget in ends:
             bins = 1 << 20
             for _ in range(2):
-                probe = GraphedRender(self.scene, cam.W, cam.H, cam.tanfovx, cam.tanfovy, self.bg,
-                                      pipeline.fov_threshold(tau, cam), sh_degree=self.sh_degree,
-                                      bin_capacity=bins, sort_capacity=8192, max_frames=1, capture=False)
+                probe = GraphedRender(self.scene, cam.W, cam.H, cam.tanfovx, cam.tanfovy, self.bg, thr,
+                                      sh_degree=self.sh_degree, row_capacity=N if budget is not None else None,
+                                      bin_capacity=bins, sort_capacity=8192, max_frames=1, capture=False, budget=budget)
                 probe.set_camera(cam)
                 probe.frame()
                 row = probe.results[0].cpu().numpy()
@@ -216,13 +250,16 @@ class HierarchyEvaluator:
         sort_cap = 32
         while sort_cap < min(2 * longest, 8192):
             sort_cap *= 2
-        return dict(row_capacity=min(int(rows * 1.25) + 1, N), bin_capacity=int(D * 1.5) + 1, sort_capacity=sort_cap)
+        row_capacity = min(int(rows * 1.25) + 1, N) if self.taus is not None else \
+            max(1, min(N, max(self.budgets) + self.scene.skybox_points))
+        return dict(row_capacity=row_capacity, bin_capacity=int(D * 1.5) + 1, sort_capacity=sort_cap)
 
     def _render_of(self, cam):
         return self.renders[(cam.W, cam.H, float(cam.tanfovx), float(cam.tanfovy))]
 
     def enqueue(self):
-        """The sweep: per camera, its inputs are copied in once, then one replay per tau.  No host synchronisation."""
+        """The sweep: per camera, its inputs are copied in once, then one replay per tau (or budget).  No host
+        synchronisation."""
         self.counter.zero_()
         last = None
         for ti, ci in self.order:
@@ -234,18 +271,24 @@ class HierarchyEvaluator:
                              None if self.exposures is None else self.exposures[ci])
                 if self.lpips is not None:
                     r.target_features()
+                if self.budgets is not None:
+                    r.set_threshold(self._floor(cam))
                 last = ci
-            r.set_threshold(pipeline.fov_threshold(self.taus[ti], cam))
+            if self.budgets is None:
+                r.set_threshold(pipeline.fov_threshold(self.taus[ti], cam))
+            else:
+                r.set_budget(self.budgets[ti])
             r.frame()
             if self.keep_images:
                 self.images[ti][ci] = r.out_image.clone()
 
-    def _exact(self, ti, ci):
+    def _exact(self, ti, ci, thr=None):
         """One frame through the exact path (host-synchronising LOD cut and num_rendered sizing) and the same metrics
-        kernel -> its row (numpy), and its LPIPS from the same kernels (None without a net)."""
+        kernel -> its row (numpy), and its LPIPS from the same kernels (None without a net).  thr: the frame's threshold
+        (a budget frame's own, as it was chosen on the device), else its tau's."""
         from diff_gaussian_rasterization import _C
         cam, r = self.cameras[ci], self._render_of(self.cameras[ci])
-        thr = pipeline.fov_threshold(self.taus[ti], cam)
+        thr = pipeline.fov_threshold(self.taus[ti], cam) if thr is None else thr
         with torch.no_grad():
             img, _, n = pipeline.render_hier_fused(self.scene, cam, self.bg, thr, self.sh_degree)
         counter = torch.zeros(1, dtype=torch.int32, device=self.dev)
@@ -276,38 +319,51 @@ class HierarchyEvaluator:
         overflow, rows, D, longest tile list), rerun = frames re-run through the exact path, flagged = their
         (tau index, camera index, capacity-mode row) -- what they needed --, images [tau][camera] when keep_images;
         with an LPIPS net also lpips={tau: mean} and lpips_rows [n_taus, n_cameras]).
-        The means are over the cameras, as render_hierarchy.py:111-119 averages them."""
-        if self.lpips is None:
-            flat = self.results[:self.n_frames].cpu().numpy()          # the one read-back of the sweep
-        else:
-            both = self._readback.cpu().numpy()
-            n = max(self.n_frames, 1)
-            flat, lp_flat = both[:n * _lib.EVAL_ROW].reshape(n, _lib.EVAL_ROW), both[n * _lib.EVAL_ROW:]
-            lp_rows = np.zeros((len(self.taus), len(self.cameras)))
-        rows = np.zeros((len(self.taus), len(self.cameras), _lib.EVAL_ROW))
+        The means are over the cameras, as render_hierarchy.py:111-119 averages them.
+        A budget sweep keys the means by budget and adds budget_rows [n_budgets, n_cameras, 4]: the threshold chosen,
+        its tau (the inverse of fov_threshold), the cut's rows and the unmet flag."""
+        n = max(self.n_frames, 1)
+        both = self._readback.cpu().numpy()                             # the one read-back of the sweep
+        flat = both[:n * _lib.EVAL_ROW].reshape(n, _lib.EVAL_ROW)
+        rest = both[n * _lib.EVAL_ROW:]
+        K, Cn = len(self.sweep), len(self.cameras)
+        if self.lpips is not None:
+            lp_flat, rest = rest[:n], rest[n:]
+            lp_rows = np.zeros((K, Cn))
+        if self.budgets is not None:
+            b_flat = rest.reshape(n, 3)
+            budget_rows = np.zeros((K, Cn, 4))
+        rows = np.zeros((K, Cn, _lib.EVAL_ROW))
         for k, (ti, ci) in enumerate(self.order):
             rows[ti, ci] = flat[k]
             if self.lpips is not None:
                 lp_rows[ti, ci] = lp_flat[k]
+            if self.budgets is not None:
+                cam = self.cameras[ci]
+                t = float(np.float32(b_flat[k, 0]))
+                budget_rows[ti, ci] = (t, t * (0.5 * cam.W) / (2 * cam.tanfovx) - 0.5, b_flat[k, 1], b_flat[k, 2])
         flagged = []
-        for ti in range(len(self.taus)):
-            for ci in range(len(self.cameras)):
+        for ti in range(K):
+            for ci in range(Cn):
                 if rows[ti, ci, 2] != 0.0:
                     flagged.append((ti, ci, rows[ti, ci].copy()))
-                    rows[ti, ci], lp = self._exact(ti, ci)
+                    thr = None if self.budgets is None else budget_rows[ti, ci, 0]
+                    rows[ti, ci], lp = self._exact(ti, ci, thr)
                     if self.lpips is not None:
                         lp_rows[ti, ci] = lp
-        psnr = {t: float(rows[ti, :, 0].mean()) for ti, t in enumerate(self.taus)}
-        ssim = {t: float(rows[ti, :, 1].mean()) for ti, t in enumerate(self.taus)}
+        psnr = {t: float(rows[ti, :, 0].mean()) for ti, t in enumerate(self.sweep)}
+        ssim = {t: float(rows[ti, :, 1].mean()) for ti, t in enumerate(self.sweep)}
         out = dict(psnr=psnr, ssim=ssim, rows=rows, rerun=len(flagged), flagged=flagged, images=self.images)
         if self.lpips is not None:
-            out["lpips"] = {t: float(lp_rows[ti].mean()) for ti, t in enumerate(self.taus)}
+            out["lpips"] = {t: float(lp_rows[ti].mean()) for ti, t in enumerate(self.sweep)}
             out["lpips_rows"] = lp_rows
+        if self.budgets is not None:
+            out["budget_rows"] = budget_rows
         return out
 
 
-def evaluate_hierarchy(scene, cameras, targets, taus, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                       bg=None, sh_degree=3, capacities=None, lpips=None):
+def evaluate_hierarchy(scene, cameras, targets, taus=None, masks=None, exposures=None, train_test_exp=False, keep_images=False,
+                       bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0):
     """The evaluation of render_hierarchy.py (render_set for every tau), sync-free.
 
     scene: pipeline.Scene with a hierarchy; cameras: pipeline.DeviceCamera per test view; targets: [3,H,W] per camera
@@ -315,8 +371,10 @@ def evaluate_hierarchy(scene, cameras, targets, taus, masks=None, exposures=None
     fallback) or None; exposures: [3,4] per camera (None entries = no exposure for that camera, as render_post does for
     a missing one) or None; train_test_exp: evaluate the right half only; capacities: dict(row_capacity, bin_capacity,
     sort_capacity) instead of the learned ones; lpips: an h3dgs.lpips.LpipsVGG net, to also report LPIPS.  Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
+    budgets (instead of taus): Gaussian budgets of the cut; per camera and budget the threshold is the finest one, no
+    finer than fov_threshold(tau_floor, camera), whose cut holds at most that many rows.
     -> see HierarchyEvaluator.finish."""
     ev = HierarchyEvaluator(scene, cameras, targets, taus, masks, exposures, train_test_exp, keep_images, bg, sh_degree,
-                            capacities, lpips)
+                            capacities, lpips, budgets, tau_floor)
     ev.enqueue()
     return ev.finish()

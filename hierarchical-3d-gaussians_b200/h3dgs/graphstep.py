@@ -311,13 +311,22 @@ class GraphedBase:
 class GraphedLodCut(GraphedBase):
     """What the hierarchy forms add: the device LOD cut.  h3dgs_lod_cut reads the threshold from threshold_dev (set_threshold
     changes it between replays), leaves the cut size in `count` on the device and marks the rows after the cut -1; the
-    skybox rows follow the cut; the raster arguments carry the fields of the gather and lerp fused into K1."""
+    skybox rows follow the cut; the raster arguments carry the fields of the gather and lerp fused into K1.
 
-    def __init__(self, scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity):
+    budget (opt-in): a Gaussian budget for the cut.  Each cut is then preceded by h3dgs_lod_budget, which writes
+    threshold_dev: the finest threshold, no finer than the one set_threshold gives (the floor), whose cut holds at most
+    the budget's rows (set_budget changes it between replays); budget_info holds {rows, unmet, nodes at or above the
+    floor, rows at the floor}.  The row capacity then defaults to budget + skybox rows."""
+
+    def __init__(self, scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget=None):
         if not scene.hier:
             raise ValueError(f"{type(self).__name__} drives the hierarchy path (LOD cut + fused gather/lerp)")
         self.N_nodes = scene.nodes.shape[0]
         _check_index_sizing(self.N_nodes, scene.means3D.shape[0])
+        if budget is not None and int(budget) < 0:
+            raise ValueError("budget must be >= 0")
+        if budget is not None and not row_capacity:
+            row_capacity = max(1, min(scene.means3D.shape[0], int(budget) + scene.skybox_points))
         super().__init__(scene, W, H, sh_degree, row_capacity, bin_capacity, sort_capacity)
         dev = self.dev
         self.S = scene.skybox_points
@@ -327,6 +336,13 @@ class GraphedLodCut(GraphedBase):
         self.count = torch.zeros(1, dtype=torch.int32, device=dev)
         self.lod_scratch = torch.empty(int(self.L.h3dgs_expand_scratch_bytes(self.N_nodes)), dtype=torch.uint8, device=dev)
         self.sky_arange = torch.arange(self.S, dtype=torch.int64, device=dev)
+        self.budget_dev = None
+        if budget is not None:
+            self.budget_dev = torch.full((1,), int(budget), dtype=torch.int32, device=dev)
+            self.floor_dev = torch.full((1,), self.threshold, dtype=torch.float32, device=dev)
+            self.budget_info = torch.zeros(4, dtype=torch.int32, device=dev)
+            self.budget_scratch = torch.empty(int(self.L.h3dgs_lod_budget_scratch_bytes(self.N_nodes)), dtype=torch.uint8,
+                                              device=dev)
 
     def _raster_args(self, tanfovx, tanfovy):
         sc = self.scene
@@ -337,6 +353,11 @@ class GraphedLodCut(GraphedBase):
 
     def _cut(self):
         sc = self.scene
+        if self.budget_dev is not None:
+            _lib.check(self.L.h3dgs_lod_budget(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.campos.data_ptr(),
+                                               self.threshold, self.floor_dev.data_ptr(), 0, self.budget_dev.data_ptr(),
+                                               self.threshold_dev.data_ptr(), self.budget_info.data_ptr(),
+                                               self.budget_scratch.data_ptr(), self._stream()))
         if self.N > self.N_nodes:
             sc.render_indices[self.N_nodes:].fill_(-1)  # the library marks [n, N_nodes); these are the skybox slots beyond
         _lib.check(self.L.h3dgs_lod_cut(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
@@ -354,9 +375,17 @@ class GraphedLodCut(GraphedBase):
             sc.num_siblings.index_fill_(0, idx, 1)
 
     def set_threshold(self, threshold):
-        """A new LOD threshold for the next step (train_post.py:66-74 draws one per step)."""
+        """A new LOD threshold for the next step (train_post.py:66-74 draws one per step); with a budget, the floor."""
         self.threshold = float(threshold)
-        self.threshold_dev.fill_(self.threshold)
+        (self.threshold_dev if self.budget_dev is None else self.floor_dev).fill_(self.threshold)
+
+    def set_budget(self, budget):
+        """A new Gaussian budget for the next cut (a form built with budget=)."""
+        if self.budget_dev is None:
+            raise ValueError("set_budget needs a form built with budget=")
+        if int(budget) < 0:
+            raise ValueError("budget must be >= 0")
+        self.budget_dev.fill_(int(budget))
 
 
 class GraphedStep(GraphedLodCut):

@@ -12,6 +12,7 @@ Used by bench.py and the GPU tests; nothing here touches oracle/.
 
 import torch
 
+from . import _lib
 from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
 from gaussian_hierarchy._C import expand_to_size, get_interpolation_weights
 
@@ -169,6 +170,30 @@ def render_hier_fused(scene, cam, bg, threshold, sh_degree=3):
                                            opacities=scene.opacities, scales=scene.scales, rotations=scene.rotations,
                                            cov3D_precomp=None)
     return img, radii, n
+
+
+def budget_threshold(scene, cam, budget, floor):
+    """The finest LOD threshold whose cut holds at most `budget` rows (skybox rows not counted), no finer than `floor`
+    -> (threshold, rows of the cut there, met).  When even the coarsest cut (at the largest finite node size) exceeds
+    the budget, that threshold comes back with met = False.  One synchronising read; sync-free forms use
+    GraphedRender(budget=...)."""
+    L = _lib.lib()
+    N, dev = scene.nodes.shape[0], scene.nodes.device
+    scratch = torch.empty(int(L.h3dgs_lod_budget_scratch_bytes(N)), dtype=torch.uint8, device=dev)
+    thr = torch.empty(1, dtype=torch.float32, device=dev)
+    info = torch.empty(4, dtype=torch.int32, device=dev)
+    _lib.check(L.h3dgs_lod_budget(N, scene.nodes.data_ptr(), scene.boxes.data_ptr(), cam.campos.data_ptr(), float(floor),
+                                  None, int(budget), None, thr.data_ptr(), info.data_ptr(), scratch.data_ptr(),
+                                  torch.cuda.current_stream(dev).cuda_stream))
+    t, i = thr.cpu(), info.cpu()
+    return float(t[0]), int(i[0]), not bool(i[1])
+
+
+def render_hier_budget(scene, cam, bg, budget, floor, sh_degree=3):
+    """render_hier_fused at budget_threshold(scene, cam, budget, floor) -> (img, radii, n, threshold, met)"""
+    threshold, _, met = budget_threshold(scene, cam, budget, floor)
+    img, radii, n = render_hier_fused(scene, cam, bg, threshold, sh_degree)
+    return img, radii, n, threshold, met
 
 
 def l1_step(scene, cam, bg, gt, threshold=None, sh_degree=3, fused=True, gt_ready=None):

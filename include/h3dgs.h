@@ -228,6 +228,20 @@ int h3dgs_lod_cut(int32_t N, const int32_t* nodes, const float* boxes, float tar
                   int32_t* render_indices, int32_t* parent_indices, int32_t* nodes_for_render_indices,
                   float* ts, int32_t* num_kids, int32_t* count, void* scratch, void* stream);
 
+/* Gaussian budget for the cut (csrc/lod_budget.cu): the smallest float t in [floor, t_max], t_max = max(floor, the
+ * largest finite node size), at which h3dgs_lod_cut's count is <= budget -- the finest cut at or above the floor that
+ * fits -- written to *threshold_out [device float], ready to be the target_size_dev of the cut.  When no t in that
+ * range fits, *threshold_out = t_max and the budget is reported unmet.  info_out [device int32 x4] = {count of the cut
+ * at *threshold_out, unmet (0/1), nodes whose size is >= floor, count of the cut at floor}.  floor_dev / budget_dev,
+ * when not NULL, are device words that override floor / budget (budget counts cut rows, skybox rows excluded; >= 0).
+ * The result depends only on the inputs: no host synchronisation, capturable.  nodes and boxes as for h3dgs_lod_cut
+ * (children contiguous at start_children, as the creator and the merger write them); scratch: 256-byte aligned,
+ * >= h3dgs_lod_budget_scratch_bytes(N). */
+int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint, float floor_size,
+                     const float* floor_dev, int32_t budget, const int32_t* budget_dev, float* threshold_out,
+                     int32_t* info_out, void* scratch, void* stream);
+size_t h3dgs_lod_budget_scratch_bytes(int32_t N);
+
 /* ---- peer memory for the tile-sharded multi-GPU mode (csrc/peer.cu) ----
  * h3dgs_peer_alloc: zero-filled device allocation that can be exported to the other ranks' processes (CUDA IPC);
  * h3dgs_peer_export / h3dgs_peer_open: 64-byte handle out / mapped pointer in (the host side exchanges the handles,
@@ -681,7 +695,7 @@ enum {
     H3DGS_STAGE_PREPROCESS = 0, H3DGS_STAGE_SCAN, H3DGS_STAGE_DUPLICATE, H3DGS_STAGE_SORT, H3DGS_STAGE_RANGES,
     H3DGS_STAGE_GATHER, H3DGS_STAGE_RENDER_FWD, H3DGS_STAGE_RENDER_BWD, H3DGS_STAGE_PREPROCESS_BWD,
     H3DGS_STAGE_LOD_CUT, H3DGS_STAGE_LOD_WEIGHTS, H3DGS_STAGE_PREPROCESS_COLOR, H3DGS_STAGE_SH_BACKWARD,
-    H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, H3DGS_STAGE_INVDEPTH_L1, H3DGS_STAGE_DENSIFY_STATS,
+    H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, H3DGS_STAGE_INVDEPTH_L1, H3DGS_STAGE_DENSIFY_STATS, H3DGS_STAGE_LOD_BUDGET,
     H3DGS_STAGE_COUNT
 };
 int h3dgs_profile_enable(int on);
