@@ -191,7 +191,7 @@ extern "C" const char* h3dgs_stage_name(int stage) {
     static const char* names[H3DGS_STAGE_COUNT] = {"preprocess", "scan", "key_emission", "sort", "identify_tile_ranges",
         "gather_records", "render_forward", "render_backward", "preprocess_backward", "lod_cut", "lod_weights",
         "preprocess_color", "sh_backward", "post_loss_backward_exposure", "invdepth_l1_grad", "densify_stats",
-        "lod_budget"};
+        "lod_budget", "lod_cull"};
     return (stage >= 0 && stage < H3DGS_STAGE_COUNT) ? names[stage] : "?";
 }
 extern "C" const char* h3dgs_last_error(void) { return g_err; }

@@ -7,6 +7,9 @@
 // target while its parent is not, or when it is too coarse but holds leaf Gaussians),
 // with an order-preserving compaction -- one kernel, one pass (lod_cut_fused_kernel).
 // HBM-bound: 28 B node + 32 B box (+ the parent's box, an L2 hit in BFS order) per node.
+//
+// With a row mask (the view cull, lod_cull.cu; NULL = every row), a node's count is the number of masked rows in its
+// range and only those rows are emitted, in order, with the fields they have without the mask.
 #include "common.cuh"
 #include "lod_size.cuh"
 #include "tma.cuh"
@@ -66,12 +69,34 @@ constexpr int kCutThreads = 256, kCutItems = 4, kCutTile = kCutThreads * kCutIte
 constexpr unsigned long long kTileAgg = 1ull << 62, kTilePrefix = 2ull << 62, kTileValue = (1ull << 62) - 1;
 constexpr size_t kCutSmem = (size_t)kCutTile * 7 * sizeof(int) + (size_t)kCutTile * 2 * sizeof(float4);
 
+// the masked rows of one node's range [start, start + range), in order, from output position off -> the next position.
+// Out of line (noinline, spelled so that the emulation's host build takes it too): the unmasked cut keeps the register
+// allocation it has without a mask.
+__device__ __attribute__((noinline)) int emit_masked(const uint8_t* __restrict__ mask, int start, int range, int off,
+                                                     int pg, int n, float tw, int kk, int* __restrict__ render_indices,
+                                                     int* __restrict__ parent_indices,
+                                                     int* __restrict__ nodes_of_render, float* __restrict__ ts,
+                                                     int* __restrict__ kids)
+{
+    for (int q = 0; q < range; q++) {
+        if (!__ldg(mask + start + q)) continue;
+        render_indices[off] = start + q;
+        parent_indices[off] = pg;
+        nodes_of_render[off] = n;
+        if (ts) ts[off] = tw;
+        if (kids) kids[off] = kk;
+        off++;
+    }
+    return off;
+}
+
 __global__ void __launch_bounds__(kCutThreads, 3)
 lod_cut_fused_kernel(int N, const int* __restrict__ nodes, const float4* __restrict__ boxes, float target,
                      const float* __restrict__ target_dev, const float* __restrict__ viewpoint,
                      unsigned long long* __restrict__ tile_state /* [tiles] zeroed */, unsigned int* __restrict__ tile_counter /* zeroed */,
                      int* __restrict__ render_indices, int* __restrict__ parent_indices, int* __restrict__ nodes_of_render,
-                     float* __restrict__ ts, int* __restrict__ kids, int* __restrict__ total)
+                     float* __restrict__ ts, int* __restrict__ kids, int* __restrict__ total,
+                     const uint8_t* __restrict__ mask /* NULL: every row */)
 {
     extern __shared__ float4 s_cut[];                         // boxes [kCutTile][2] | nodes [kCutTile][7]
     __shared__ uint64_t s_bar[2];
@@ -134,6 +159,14 @@ lod_cut_fused_kernel(int N, const int* __restrict__ nodes, const float4* __restr
         }
         cnt[k] = count;
         sum += count;
+    }
+    if (mask) {                                               // the masked rows of each range: [start, start + count)
+        sum = 0;
+#pragma unroll
+        for (int k = 0; k < kCutItems; k++) {
+            if (cnt[k] > 0) cnt[k] = masked_rows(mask, s_node[7 * (tid * kCutItems + k) + 2], cnt[k]);
+            sum += cnt[k];
+        }
     }
     // ---- one block-wide exclusive scan of the thread sums ----
     int incl = sum;
@@ -198,6 +231,13 @@ lod_cut_fused_kernel(int N, const int* __restrict__ nodes, const float4* __restr
             const float diff = psize[k] - st;
             if (diff > 0) tw = fmaxf(1.0f - (fmaxf(0.0f, target - st) / diff), 0.0f);
         }
+        if (mask) {                                           // the masked rows of the node's range, in order
+            const int* nd = s_node + 7 * j;
+            const int range = size[k] >= target ? nd[3] : nd[3] + (nd[0] != 0 ? nd[4] : 0);
+            off = emit_masked(mask, start, range, off, pg[k], n, tw, kk[k], render_indices, parent_indices,
+                              nodes_of_render, ts, kids);
+            continue;
+        }
         for (int q = 0; q < cnt[k]; q++) {
             render_indices[off + q] = start + q;
             parent_indices[off + q] = pg[k];
@@ -229,7 +269,8 @@ static bool boxes_misaligned(const float* boxes, const char* who) {
 // one launch of the single-pass cut; scratch holds the tile status words and the tile counter
 static int launch_cut(int N, const int32_t* nodes, const float* boxes, float target_size, const float* target_size_dev,
                       const float* viewpoint, int32_t* render_indices, int32_t* parent_indices, int32_t* nodes_for_render_indices,
-                      float* ts, int32_t* num_kids, int32_t* total, void* scratch, cudaStream_t s)
+                      float* ts, int32_t* num_kids, int32_t* total, void* scratch, cudaStream_t s,
+                      const uint8_t* mask = nullptr)
 {
     const int tiles = (N + kCutTile - 1) / kCutTile;
     unsigned long long* state = (unsigned long long*)scratch;
@@ -244,7 +285,7 @@ static int launch_cut(int N, const int32_t* nodes, const float* boxes, float tar
     }
     lod_cut_fused_kernel<<<tiles, kCutThreads, kCutSmem, s>>>(N, nodes, (const float4*)boxes, target_size, target_size_dev, viewpoint, state,
                                                        counter, render_indices, parent_indices, nodes_for_render_indices, ts,
-                                                       num_kids, total);
+                                                       num_kids, total, mask);
     H3_LAUNCHED("lod_cut_fused", 0, s);
     return H3DGS_OK;
 }
@@ -269,21 +310,39 @@ extern "C" int h3dgs_expand_to_size(int32_t N, const int32_t* nodes, const float
     return *static_cast<const int*>(pin);
 }
 
-extern "C" int h3dgs_lod_cut(int32_t N, const int32_t* nodes, const float* boxes, float target_size,
-                             const float* target_size_dev, const float* viewpoint, int32_t* render_indices, int32_t* parent_indices,
-                             int32_t* nodes_for_render_indices, float* ts, int32_t* num_kids, int32_t* count,
-                             void* scratch, void* stream)
+static int lod_cut(const char* who, int32_t N, const int32_t* nodes, const float* boxes, float target_size,
+                   const float* target_size_dev, const float* viewpoint, int32_t* render_indices, int32_t* parent_indices,
+                   int32_t* nodes_for_render_indices, float* ts, int32_t* num_kids, int32_t* count, void* scratch,
+                   void* stream, const uint8_t* mask)
 {
-    if (N <= 0) { set_error("lod_cut: empty hierarchy"); return H3DGS_EINVAL; }
+    if (N <= 0) { set_error("%s: empty hierarchy", who); return H3DGS_EINVAL; }
     if (!nodes || !boxes || !viewpoint || !render_indices || !parent_indices || !nodes_for_render_indices || !ts ||
-        !num_kids || !count || !scratch) { set_error("lod_cut: NULL argument"); return H3DGS_EINVAL; }
-    if (boxes_misaligned(boxes, "lod_cut")) return H3DGS_EINVAL;
+        !num_kids || !count || !scratch) { set_error("%s: NULL argument", who); return H3DGS_EINVAL; }
+    if (boxes_misaligned(boxes, who)) return H3DGS_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope prof(H3DGS_STAGE_LOD_CUT, s);
     // rows after the cut: index -1 = "skip" for the rasterizer (the head is overwritten by the cut)
     H3_CUDA(cudaMemsetAsync(render_indices, 0xFF, (size_t)N * sizeof(int32_t), s));
     return launch_cut(N, nodes, boxes, target_size, target_size_dev, viewpoint, render_indices, parent_indices,
-                      nodes_for_render_indices, ts, num_kids, count, scratch, s);
+                      nodes_for_render_indices, ts, num_kids, count, scratch, s, mask);
+}
+
+extern "C" int h3dgs_lod_cut(int32_t N, const int32_t* nodes, const float* boxes, float target_size,
+                             const float* target_size_dev, const float* viewpoint, int32_t* render_indices, int32_t* parent_indices,
+                             int32_t* nodes_for_render_indices, float* ts, int32_t* num_kids, int32_t* count,
+                             void* scratch, void* stream)
+{
+    return lod_cut("lod_cut", N, nodes, boxes, target_size, target_size_dev, viewpoint, render_indices, parent_indices,
+                   nodes_for_render_indices, ts, num_kids, count, scratch, stream, nullptr);
+}
+
+extern "C" int h3dgs_lod_cut_masked(int32_t N, const int32_t* nodes, const float* boxes, float target_size,
+                                    const float* target_size_dev, const float* viewpoint, const uint8_t* row_mask,
+                                    int32_t* render_indices, int32_t* parent_indices, int32_t* nodes_for_render_indices,
+                                    float* ts, int32_t* num_kids, int32_t* count, void* scratch, void* stream)
+{
+    return lod_cut("lod_cut_masked", N, nodes, boxes, target_size, target_size_dev, viewpoint, render_indices,
+                   parent_indices, nodes_for_render_indices, ts, num_kids, count, scratch, stream, row_mask);
 }
 
 extern "C" int h3dgs_get_interpolation_weights(int32_t n, const int32_t* node_indices, float target_size,

@@ -17,6 +17,9 @@
 // smallest feasible x below t_max (R need not be monotone, so every run is a candidate: one atomicMax over run
 // positions, whose result does not depend on the order of the atomics), else t_max with the "unmet" flag.
 //
+// With the view cull's row mask (lod_cull.cu), cl and cm become the node's masked leaf and merged rows (vl, vm): the
+// masked cut has the same per-node predicate with those counts, so the argument above holds unchanged.
+//
 // Launches: a memset, the key kernel, cub's radix sort and inclusive scan, the selection kernel and a one-thread
 // finisher; every size is fixed by N, floor and budget are read on the device, so the call is capturable.
 #include <cub/cub.cuh>
@@ -34,7 +37,7 @@ enum { kBudgetKept = 0, kBudgetBest, kBudgetFirst, kBudgetInf, kBudgetWords };
 __global__ void __launch_bounds__(kBudgetThreads)
 budget_keys_kernel(int N, const int* __restrict__ nodes, const float4* __restrict__ boxes, float floor_t,
                    const float* __restrict__ floor_dev, const float* __restrict__ viewpoint, uint32_t* __restrict__ keys,
-                   int* __restrict__ weights, int* __restrict__ small)
+                   int* __restrict__ weights, int* __restrict__ small, const uint8_t* __restrict__ mask /* NULL: every row */)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (floor_dev) floor_t = *floor_dev;
@@ -48,16 +51,20 @@ budget_keys_kernel(int N, const int* __restrict__ nodes, const float4* __restric
         if (s >= floor_t) {
             kept = true;
             const int parent = nd[1];
-            w = nd[3];
+            w = mask ? masked_rows(mask, nd[2], nd[3]) : nd[3];
             if (parent != -1) {
                 const float q = box_size(__ldg(boxes + 2 * (size_t)parent), __ldg(boxes + 2 * (size_t)parent + 1), vx, vy, vz);
-                if (!(s >= q) && q == q) w = nd[0] != 0 ? -nd[4] : 0;
+                if (!(s >= q) && q == q)
+                    w = nd[0] != 0 ? -(mask ? masked_rows(mask, nd[2] + nd[3], nd[4]) : nd[4]) : 0;
             }
             const int first = nd[5], nk = nd[6];
             for (int c = first; c < first + nk; c++) {           // the children's terms at this node's size
                 const int* cd = nodes + 7 * (size_t)c;
                 const float sc = box_size(__ldg(boxes + 2 * (size_t)c), __ldg(boxes + 2 * (size_t)c + 1), vx, vy, vz);
-                if (!(sc >= s)) w += cd[3] + (cd[0] != 0 ? cd[4] : 0);
+                if (!(sc >= s)) {
+                    const int rows = cd[3] + (cd[0] != 0 ? cd[4] : 0);
+                    w += mask ? masked_rows(mask, cd[2], rows) : rows;
+                }
             }
             key = ~f2key(s == 0.0f ? 0.0f : s);                  // -0 and +0 are one size; ascending = sizes descending
         }
@@ -144,18 +151,18 @@ using namespace h3dgs;
 
 extern "C" size_t h3dgs_lod_budget_scratch_bytes(int32_t N) { return budget_layout(N > 0 ? N : 1).total; }
 
-extern "C" int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint, float floor_size,
-                                const float* floor_dev, int32_t budget, const int32_t* budget_dev, float* threshold_out,
-                                int32_t* info_out, void* scratch, void* stream)
+static int lod_budget(const char* who, int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint,
+                      float floor_size, const float* floor_dev, int32_t budget, const int32_t* budget_dev,
+                      float* threshold_out, int32_t* info_out, void* scratch, void* stream, const uint8_t* mask)
 {
-    if (N <= 0) { set_error("lod_budget: empty hierarchy"); return H3DGS_EINVAL; }
+    if (N <= 0) { set_error("%s: empty hierarchy", who); return H3DGS_EINVAL; }
     if (!nodes || !boxes || !viewpoint || !threshold_out || !info_out || !scratch) {
-        set_error("lod_budget: NULL argument");
+        set_error("%s: NULL argument", who);
         return H3DGS_EINVAL;
     }
-    if ((((uintptr_t)boxes) & 15) != 0) { set_error("lod_budget: boxes must be 16-byte aligned (got %p)", (const void*)boxes); return H3DGS_EINVAL; }
-    if ((((uintptr_t)scratch) & 255) != 0) { set_error("lod_budget: scratch must be 256-byte aligned (got %p)", scratch); return H3DGS_EINVAL; }
-    if (!budget_dev && budget < 0) { set_error("lod_budget: negative budget %d", budget); return H3DGS_EINVAL; }
+    if ((((uintptr_t)boxes) & 15) != 0) { set_error("%s: boxes must be 16-byte aligned (got %p)", who, (const void*)boxes); return H3DGS_EINVAL; }
+    if ((((uintptr_t)scratch) & 255) != 0) { set_error("%s: scratch must be 256-byte aligned (got %p)", who, scratch); return H3DGS_EINVAL; }
+    if (!budget_dev && budget < 0) { set_error("%s: negative budget %d", who, budget); return H3DGS_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope prof(H3DGS_STAGE_LOD_BUDGET, s);
     const BudgetLayout l = budget_layout(N);
@@ -167,7 +174,7 @@ extern "C" int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* bo
     const int blocks = (N + kBudgetThreads - 1) / kBudgetThreads;
     H3_CUDA(cudaMemsetAsync(small, 0, kBudgetWords * sizeof(int), s));
     budget_keys_kernel<<<blocks, kBudgetThreads, 0, s>>>(N, nodes, (const float4*)boxes, floor_size, floor_dev, viewpoint,
-                                                         keys_in, w_in, small);
+                                                         keys_in, w_in, small, mask);
     H3_LAUNCHED("lod_budget_keys", 0, s);
     H3_CUDA(cub::DeviceRadixSort::SortPairs(base + l.temp, temp_bytes, keys_in, keys_out, w_in, w_out, N, 0, 32, s));
     H3_LAUNCHED("lod_budget_sort", 0, s);
@@ -181,4 +188,21 @@ extern "C" int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* bo
                                          threshold_out, info_out);
     H3_LAUNCHED("lod_budget_finish", 0, s);
     return H3DGS_OK;
+}
+
+extern "C" int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint, float floor_size,
+                                const float* floor_dev, int32_t budget, const int32_t* budget_dev, float* threshold_out,
+                                int32_t* info_out, void* scratch, void* stream)
+{
+    return lod_budget("lod_budget", N, nodes, boxes, viewpoint, floor_size, floor_dev, budget, budget_dev, threshold_out,
+                      info_out, scratch, stream, nullptr);
+}
+
+extern "C" int h3dgs_lod_budget_masked(int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint,
+                                       const uint8_t* row_mask, float floor_size, const float* floor_dev, int32_t budget,
+                                       const int32_t* budget_dev, float* threshold_out, int32_t* info_out, void* scratch,
+                                       void* stream)
+{
+    return lod_budget("lod_budget_masked", N, nodes, boxes, viewpoint, floor_size, floor_dev, budget, budget_dev,
+                      threshold_out, info_out, scratch, stream, row_mask);
 }

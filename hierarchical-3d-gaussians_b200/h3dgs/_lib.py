@@ -18,7 +18,8 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 EXPORTS = [
     "h3dgs_rasterize_forward", "h3dgs_rasterize_backward", "h3dgs_backward_scratch_bytes", "h3dgs_mark_visible",
     "h3dgs_state_layout", "h3dgs_expand_to_size", "h3dgs_expand_scratch_bytes", "h3dgs_get_interpolation_weights",
-    "h3dgs_lod_cut", "h3dgs_lod_budget", "h3dgs_lod_budget_scratch_bytes",
+    "h3dgs_lod_cut", "h3dgs_lod_budget", "h3dgs_lod_budget_scratch_bytes", "h3dgs_lod_cull_mask", "h3dgs_lod_cut_masked",
+    "h3dgs_lod_budget_masked",
     "h3dgs_last_error", "h3dgs_version", "h3dgs_launch_count",
     "h3dgs_profile_enable", "h3dgs_profile_reset", "h3dgs_profile_read", "h3dgs_stage_name",
     "h3dgs_l1_ssim_forward", "h3dgs_l1_ssim_backward", "h3dgs_l1_loss_grad", "h3dgs_l1_loss_grad_peer", "h3dgs_step_status", "h3dgs_sparse_adam",
@@ -185,6 +186,15 @@ def bind(l):
         l.h3dgs_lod_budget_scratch_bytes.argtypes = [C.c_int32]
         l.h3dgs_lod_budget.restype = C.c_int
         l.h3dgs_lod_budget.argtypes = [C.c_int32] + [C.c_void_p] * 3 + [C.c_float, C.c_void_p, C.c_int32] + [C.c_void_p] * 5
+        l.h3dgs_lod_budget_masked.restype = C.c_int
+        l.h3dgs_lod_budget_masked.argtypes = [C.c_int32] + [C.c_void_p] * 4 + [C.c_float, C.c_void_p, C.c_int32] + \
+            [C.c_void_p] * 5
+    l.h3dgs_lod_cut_masked.restype = C.c_int
+    l.h3dgs_lod_cut_masked.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_float] + [C.c_void_p] * 11
+    if hasattr(l, "h3dgs_lod_cull_mask"):        # view cull (an emulation build has it when it compiles lod_cull.cu)
+        l.h3dgs_lod_cull_mask.restype = C.c_int
+        l.h3dgs_lod_cull_mask.argtypes = [C.c_int32] + [C.c_void_p] * 4 + [C.c_float] + [C.c_void_p] * 2 + \
+            [C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
     if hasattr(l, "h3dgs_eval_metrics"):         # evaluation metrics (an emulation build has it when it compiles metrics.cu)
         l.h3dgs_eval_metrics.restype = C.c_int
         l.h3dgs_eval_metrics.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] + [C.c_void_p] * 3 + \
@@ -296,7 +306,7 @@ def launch_count():
     return int(lib().h3dgs_launch_count())
 
 
-STAGES = 17
+STAGES = 18
 
 
 def profile_enable(on=True):

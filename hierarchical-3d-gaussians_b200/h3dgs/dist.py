@@ -134,7 +134,9 @@ class TileSharder:
     def __init__(self, world, rank, device, group=None):
         self.world, self.rank, self.device, self.group = world, rank, device, group
 
-    def render(self, scene, cam, bg, threshold=None, sh_degree=3):
+    def render(self, scene, cam, bg, threshold=None, sh_degree=3, cull=False):
+        if cull:
+            raise ValueError("cull=True runs on one GPU: the tile-sharded forms take the unculled cut")
         if scene.hier:
             # fused form: the cut gather + parent lerp run inside K1/K9 (full arrays + indices)
             n, P = pipeline.fused_cut(scene, cam, threshold)
@@ -148,9 +150,9 @@ class TileSharder:
         img, radii = _ShardedRasterize.apply(means, shs, opac, scales, rots, rs, self.world, self.rank, self.group)
         return img, radii, n
 
-    def l1_step(self, scene, cam, bg, gt, threshold=None, sh_degree=3, gt_ready=None):
+    def l1_step(self, scene, cam, bg, gt, threshold=None, sh_degree=3, gt_ready=None, cull=False):
         scene.zero_grad()
-        img, radii, n = self.render(scene, cam, bg, threshold, sh_degree)
+        img, radii, n = self.render(scene, cam, bg, threshold, sh_degree, cull)
         if gt_ready is not None:
             torch.cuda.current_stream().wait_event(gt_ready)
         loss = (img - gt).abs().mean()

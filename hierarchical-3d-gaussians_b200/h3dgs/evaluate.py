@@ -53,13 +53,16 @@ class GraphedRender(GraphedLodCut):
 
     budget: a Gaussian budget (GraphedLodCut): the cut's threshold is then chosen on the device, no finer than the
     threshold (the floor; set_threshold), and each frame also stores [threshold, rows, unmet] at its slot of
-    `budget_values`."""
+    `budget_values`.
+
+    cull: the view-culled cut (GraphedLodCut): the same image, with only the rows that can reach it; the frame's rows
+    (and a budget's) are the visible rows."""
 
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None, bin_capacity=1 << 22,
                  sort_capacity=4096, exposure=False, mask=False, train_test_exp=False, keep_image=False, results=None,
                  counter=None, max_frames=1024, capture=True, lpips=None, lpips_values=None, budget=None,
-                 budget_values=None):
-        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget)
+                 budget_values=None, cull=False):
+        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget, cull)
         dev, H, W = self.dev, self.H, self.W
         self.image = self._zeros(3, H, W)
         self._init_inputs(exposure, mask)
@@ -158,10 +161,13 @@ class HierarchyEvaluator:
 
     With budgets (and taus None) the sweep runs over Gaussian budgets instead of taus: each frame's threshold is the finest
     one, no finer than fov_threshold(tau_floor, camera), whose cut holds at most the budget's rows (GraphedRender's
-    budget=), and the frame's [threshold, rows, unmet] travel in the same read-back."""
+    budget=), and the frame's [threshold, rows, unmet] travel in the same read-back.
+
+    cull: every frame takes the view-culled cut (GraphedRender's cull=): the same images and metrics, and a budget counts
+    the visible rows only."""
 
     def __init__(self, scene, cameras, targets, taus, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                 bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0):
+                 bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0, cull=False):
         if not scene.hier:
             raise ValueError("evaluate_hierarchy needs a hierarchy scene")
         if (taus is None) == (budgets is None):
@@ -175,6 +181,7 @@ class HierarchyEvaluator:
         self.taus = None if taus is None else [float(t) for t in taus]
         self.budgets = None if budgets is None else [int(b) for b in budgets]
         self.tau_floor = float(tau_floor)
+        self.cull = bool(cull)
         self.sweep = self.taus if budgets is None else self.budgets       # what a frame's first index runs over
         self.sh_degree, self.train_test_exp, self.keep_images = int(sh_degree), bool(train_test_exp), bool(keep_images)
         dev = scene.means3D.device
@@ -217,7 +224,7 @@ class HierarchyEvaluator:
                              sh_degree=self.sh_degree, exposure=self.exposures is not None, mask=self.masks is not None,
                              train_test_exp=self.train_test_exp, keep_image=self.keep_images, results=self.results,
                              counter=self.counter, lpips=self.lpips, lpips_values=self.lpips_values, budget=budget,
-                             budget_values=self.budget_values, **kw)
+                             budget_values=self.budget_values, cull=self.cull, **kw)
 
     def _learn_capacities(self, cam):
         """Eager capacity-mode frames of the first view at the smallest and at the largest tau, with every row and a
@@ -238,7 +245,8 @@ class HierarchyEvaluator:
             for _ in range(2):
                 probe = GraphedRender(self.scene, cam.W, cam.H, cam.tanfovx, cam.tanfovy, self.bg, thr,
                                       sh_degree=self.sh_degree, row_capacity=N if budget is not None else None,
-                                      bin_capacity=bins, sort_capacity=8192, max_frames=1, capture=False, budget=budget)
+                                      bin_capacity=bins, sort_capacity=8192, max_frames=1, capture=False, budget=budget,
+                                      cull=self.cull)
                 probe.set_camera(cam)
                 probe.frame()
                 row = probe.results[0].cpu().numpy()
@@ -290,7 +298,7 @@ class HierarchyEvaluator:
         cam, r = self.cameras[ci], self._render_of(self.cameras[ci])
         thr = pipeline.fov_threshold(self.taus[ti], cam) if thr is None else thr
         with torch.no_grad():
-            img, _, n = pipeline.render_hier_fused(self.scene, cam, self.bg, thr, self.sh_degree)
+            img, _, n = pipeline.render_hier_fused(self.scene, cam, self.bg, thr, self.sh_degree, self.cull)
         counter = torch.zeros(1, dtype=torch.int32, device=self.dev)
         results = torch.zeros((1, _lib.EVAL_ROW), dtype=torch.float64, device=self.dev)
         out = torch.zeros((3, cam.H, cam.W - r.x0), device=self.dev) if self.keep_images else None
@@ -363,7 +371,7 @@ class HierarchyEvaluator:
 
 
 def evaluate_hierarchy(scene, cameras, targets, taus=None, masks=None, exposures=None, train_test_exp=False, keep_images=False,
-                       bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0):
+                       bg=None, sh_degree=3, capacities=None, lpips=None, budgets=None, tau_floor=0.0, cull=False):
     """The evaluation of render_hierarchy.py (render_set for every tau), sync-free.
 
     scene: pipeline.Scene with a hierarchy; cameras: pipeline.DeviceCamera per test view; targets: [3,H,W] per camera
@@ -373,8 +381,10 @@ def evaluate_hierarchy(scene, cameras, targets, taus=None, masks=None, exposures
     sort_capacity) instead of the learned ones; lpips: an h3dgs.lpips.LpipsVGG net, to also report LPIPS.  Per camera and tau the LOD threshold is pipeline.fov_threshold(tau, camera) (render_hierarchy.py:55-56).
     budgets (instead of taus): Gaussian budgets of the cut; per camera and budget the threshold is the finest one, no
     finer than fov_threshold(tau_floor, camera), whose cut holds at most that many rows.
+    cull: cut only the rows that can reach each camera's image (the same images and metrics; a budget then counts the
+    visible rows).
     -> see HierarchyEvaluator.finish."""
     ev = HierarchyEvaluator(scene, cameras, targets, taus, masks, exposures, train_test_exp, keep_images, bg, sh_degree,
-                            capacities, lpips, budgets, tau_floor)
+                            capacities, lpips, budgets, tau_floor, cull)
     ev.enqueue()
     return ev.finish()

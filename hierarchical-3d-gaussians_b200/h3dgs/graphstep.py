@@ -316,9 +316,14 @@ class GraphedLodCut(GraphedBase):
     budget (opt-in): a Gaussian budget for the cut.  Each cut is then preceded by h3dgs_lod_budget, which writes
     threshold_dev: the finest threshold, no finer than the one set_threshold gives (the floor), whose cut holds at most
     the budget's rows (set_budget changes it between replays); budget_info holds {rows, unmet, nodes at or above the
-    floor, rows at the floor}.  The row capacity then defaults to budget + skybox rows."""
+    floor, rows at the floor}.  The row capacity then defaults to budget + skybox rows.
 
-    def __init__(self, scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget=None):
+    cull (opt-in): the view cull.  Each frame then starts with h3dgs_lod_cull_mask, the row mask of the hierarchy rows
+    that can reach the camera's image, and the budget (if any) and the cut take only those rows: `count` and
+    budget_info's rows are the visible rows, the image is the unculled one bit for bit.  Skybox rows are not culled."""
+
+    def __init__(self, scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, budget=None,
+                 cull=False):
         if not scene.hier:
             raise ValueError(f"{type(self).__name__} drives the hierarchy path (LOD cut + fused gather/lerp)")
         self.N_nodes = scene.nodes.shape[0]
@@ -343,6 +348,7 @@ class GraphedLodCut(GraphedBase):
             self.budget_info = torch.zeros(4, dtype=torch.int32, device=dev)
             self.budget_scratch = torch.empty(int(self.L.h3dgs_lod_budget_scratch_bytes(self.N_nodes)), dtype=torch.uint8,
                                               device=dev)
+        self.cull_mask = torch.zeros(self.N, dtype=torch.uint8, device=dev) if cull else None
 
     def _raster_args(self, tanfovx, tanfovy):
         sc = self.scene
@@ -352,19 +358,37 @@ class GraphedLodCut(GraphedBase):
         return a
 
     def _cut(self):
-        sc = self.scene
+        sc, m = self.scene, self.cull_mask
+        if m is not None:
+            a = self.args                               # the rows, camera and sizes K1 draws with
+            _lib.check(self.L.h3dgs_lod_cull_mask(self.N_nodes, sc.nodes.data_ptr(), a.means3D, a.scales, a.rotations,
+                                                  a.scale_modifier, self.view.data_ptr(), self.proj.data_ptr(),
+                                                  a.image_width, a.image_height, a.tanfovx, a.tanfovy, m.data_ptr(),
+                                                  self._stream()))
         if self.budget_dev is not None:
-            _lib.check(self.L.h3dgs_lod_budget(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.campos.data_ptr(),
-                                               self.threshold, self.floor_dev.data_ptr(), 0, self.budget_dev.data_ptr(),
-                                               self.threshold_dev.data_ptr(), self.budget_info.data_ptr(),
-                                               self.budget_scratch.data_ptr(), self._stream()))
+            if m is None:
+                _lib.check(self.L.h3dgs_lod_budget(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(),
+                                                   self.campos.data_ptr(), self.threshold, self.floor_dev.data_ptr(), 0,
+                                                   self.budget_dev.data_ptr(), self.threshold_dev.data_ptr(),
+                                                   self.budget_info.data_ptr(), self.budget_scratch.data_ptr(), self._stream()))
+            else:
+                _lib.check(self.L.h3dgs_lod_budget_masked(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(),
+                                                          self.campos.data_ptr(), m.data_ptr(), self.threshold,
+                                                          self.floor_dev.data_ptr(), 0, self.budget_dev.data_ptr(),
+                                                          self.threshold_dev.data_ptr(), self.budget_info.data_ptr(),
+                                                          self.budget_scratch.data_ptr(), self._stream()))
         if self.N > self.N_nodes:
             sc.render_indices[self.N_nodes:].fill_(-1)  # the library marks [n, N_nodes); these are the skybox slots beyond
-        _lib.check(self.L.h3dgs_lod_cut(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
-                                        self.threshold_dev.data_ptr(), self.campos.data_ptr(), sc.render_indices.data_ptr(),
-                                        sc.parent_indices.data_ptr(), sc.nodes_for_render.data_ptr(),
-                                        sc.interpolation_weights.data_ptr(), sc.num_siblings.data_ptr(),
-                                        self.count.data_ptr(), self.lod_scratch.data_ptr(), self._stream()))
+        cut_args = (sc.render_indices.data_ptr(), sc.parent_indices.data_ptr(), sc.nodes_for_render.data_ptr(),
+                    sc.interpolation_weights.data_ptr(), sc.num_siblings.data_ptr(), self.count.data_ptr(),
+                    self.lod_scratch.data_ptr(), self._stream())
+        if m is None:
+            _lib.check(self.L.h3dgs_lod_cut(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
+                                            self.threshold_dev.data_ptr(), self.campos.data_ptr(), *cut_args))
+        else:
+            _lib.check(self.L.h3dgs_lod_cut_masked(self.N_nodes, sc.nodes.data_ptr(), sc.boxes.data_ptr(), self.threshold,
+                                                   self.threshold_dev.data_ptr(), self.campos.data_ptr(), m.data_ptr(),
+                                                   *cut_args))
         if self.S:
             # skybox rows follow the cut as their own parents with t = 1, kids = 1 (render_post :220-234);
             # a cut so large that they would not fit is reported as a row overflow by status()
@@ -395,8 +419,10 @@ class GraphedStep(GraphedLodCut):
 
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=3, row_capacity=None,
                  bin_capacity=1 << 22, sort_capacity=4096, world=1, rank=0, group=None, capture=True, peer=False,
-                 cyclic_log2=12):
-        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity)
+                 cyclic_log2=12, cull=False):
+        if cull and int(world) > 1:
+            raise ValueError("cull=True runs on one GPU: the multi-GPU forms take the unculled cut")
+        super().__init__(scene, W, H, bg, threshold, sh_degree, row_capacity, bin_capacity, sort_capacity, cull=cull)
         self.world, self.rank, self.group = int(world), int(rank), group
         self.peer = bool(peer) and self.world > 1
         if self.peer and (self.world & (self.world - 1) or self.world > _lib.MAX_PEERS):

@@ -145,10 +145,39 @@ def render_hier(scene, cam, bg, threshold, sh_degree=3):
     return img, radii, n
 
 
-def fused_cut(scene, cam, threshold):
+def cull_mask(scene, cam, out=None):
+    """The view cull's row mask (h3dgs_lod_cull_mask) -> uint8 [rows] on the device: 1 for every hierarchy row the
+    rasterizer could draw from `cam` at some lerp weight, whatever the threshold; skybox rows are not written."""
+    L = _lib.lib()
+    if out is None:
+        out = torch.zeros(scene.means3D.shape[0], dtype=torch.uint8, device=scene.means3D.device)
+    _lib.check(L.h3dgs_lod_cull_mask(scene.nodes.shape[0], scene.nodes.data_ptr(), scene.means3D.data_ptr(),
+                                     scene.scales.data_ptr(), scene.rotations.data_ptr(), 1.0, cam.viewmatrix.data_ptr(),
+                                     cam.projmatrix.data_ptr(), cam.W, cam.H, float(cam.tanfovx), float(cam.tanfovy),
+                                     out.data_ptr(), torch.cuda.current_stream(out.device).cuda_stream))
+    return out
+
+
+def _culled_cut(scene, cam, threshold):
+    """the cut under the view cull's mask (h3dgs_lod_cut_masked), weights included -> n; one synchronising read"""
+    L = _lib.lib()
+    N, dev = scene.nodes.shape[0], scene.nodes.device
+    mask = cull_mask(scene, cam)
+    count = torch.zeros(1, dtype=torch.int32, device=dev)
+    scratch = torch.empty(int(L.h3dgs_expand_scratch_bytes(N)), dtype=torch.uint8, device=dev)
+    _lib.check(L.h3dgs_lod_cut_masked(N, scene.nodes.data_ptr(), scene.boxes.data_ptr(), float(threshold), None,
+                                      cam.campos.data_ptr(), mask.data_ptr(), scene.render_indices.data_ptr(),
+                                      scene.parent_indices.data_ptr(), scene.nodes_for_render.data_ptr(),
+                                      scene.interpolation_weights.data_ptr(), scene.num_siblings.data_ptr(),
+                                      count.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    return int(count.item())
+
+
+def fused_cut(scene, cam, threshold, cull=False):
     """LOD cut for the fused form -> (n cut rows, P rows to rasterize): the skybox rows follow the
-    cut in render_indices/parent_indices as their own parents with t = 1, kids = 1."""
-    n = lod_cut(scene, cam, threshold)
+    cut in render_indices/parent_indices as their own parents with t = 1, kids = 1.
+    cull: keep only the cut rows that can reach cam's image (cull_mask); the image is the same."""
+    n = _culled_cut(scene, cam, threshold) if cull else lod_cut(scene, cam, threshold)
     S = scene.skybox_points
     if S:
         scene.render_indices[n:n + S] = scene.skybox_inds
@@ -157,12 +186,13 @@ def fused_cut(scene, cam, threshold):
     return n, n + S
 
 
-def render_hier_fused(scene, cam, bg, threshold, sh_degree=3):
+def render_hier_fused(scene, cam, bg, threshold, sh_degree=3, cull=False):
     """Same result as render_hier, but the cut gather + parent lerp (and the gradient scatter in
     backward) run inside K1/K9 through the settings' render_indices/parent_indices fields instead
     of ~25 PyTorch kernels with full-size temporaries (SURVEY.md 8f-1).  Skybox rows are appended to
-    the cut as indices that are their own parent with t = 1 (x = 1*x exactly, as in render_post)."""
-    n, P = fused_cut(scene, cam, threshold)
+    the cut as indices that are their own parent with t = 1 (x = 1*x exactly, as in render_post).
+    cull: the view-culled cut (fused_cut); the image is bit-identical, n counts the culled cut's rows."""
+    n, P = fused_cut(scene, cam, threshold, cull)
     rs = make_settings(scene, cam, bg, sh_degree, ts=scene.interpolation_weights, kids=scene.num_siblings,
                        ridx=scene.render_indices[:P], pidx=scene.parent_indices[:P])
     means2D = torch.zeros((P, 3), device=scene.means3D.device, requires_grad=scene.means3D.requires_grad)
@@ -172,27 +202,28 @@ def render_hier_fused(scene, cam, bg, threshold, sh_degree=3):
     return img, radii, n
 
 
-def budget_threshold(scene, cam, budget, floor):
+def budget_threshold(scene, cam, budget, floor, cull=False):
     """The finest LOD threshold whose cut holds at most `budget` rows (skybox rows not counted), no finer than `floor`
     -> (threshold, rows of the cut there, met).  When even the coarsest cut (at the largest finite node size) exceeds
-    the budget, that threshold comes back with met = False.  One synchronising read; sync-free forms use
-    GraphedRender(budget=...)."""
+    the budget, that threshold comes back with met = False.  cull: count only the rows that can reach cam's image
+    (cull_mask), the rows the culled cut keeps.  One synchronising read; sync-free forms use GraphedRender(budget=...)."""
     L = _lib.lib()
     N, dev = scene.nodes.shape[0], scene.nodes.device
     scratch = torch.empty(int(L.h3dgs_lod_budget_scratch_bytes(N)), dtype=torch.uint8, device=dev)
     thr = torch.empty(1, dtype=torch.float32, device=dev)
     info = torch.empty(4, dtype=torch.int32, device=dev)
-    _lib.check(L.h3dgs_lod_budget(N, scene.nodes.data_ptr(), scene.boxes.data_ptr(), cam.campos.data_ptr(), float(floor),
-                                  None, int(budget), None, thr.data_ptr(), info.data_ptr(), scratch.data_ptr(),
-                                  torch.cuda.current_stream(dev).cuda_stream))
+    mask = cull_mask(scene, cam) if cull else None
+    _lib.check(L.h3dgs_lod_budget_masked(N, scene.nodes.data_ptr(), scene.boxes.data_ptr(), cam.campos.data_ptr(),
+                                         _lib.ptr(mask), float(floor), None, int(budget), None, thr.data_ptr(),
+                                         info.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
     t, i = thr.cpu(), info.cpu()
     return float(t[0]), int(i[0]), not bool(i[1])
 
 
-def render_hier_budget(scene, cam, bg, budget, floor, sh_degree=3):
-    """render_hier_fused at budget_threshold(scene, cam, budget, floor) -> (img, radii, n, threshold, met)"""
-    threshold, _, met = budget_threshold(scene, cam, budget, floor)
-    img, radii, n = render_hier_fused(scene, cam, bg, threshold, sh_degree)
+def render_hier_budget(scene, cam, bg, budget, floor, sh_degree=3, cull=False):
+    """render_hier_fused at budget_threshold(scene, cam, budget, floor, cull) -> (img, radii, n, threshold, met)"""
+    threshold, _, met = budget_threshold(scene, cam, budget, floor, cull)
+    img, radii, n = render_hier_fused(scene, cam, bg, threshold, sh_degree, cull)
     return img, radii, n, threshold, met
 
 

@@ -138,11 +138,11 @@ class GraphedPostStep(GraphedStep):
 
     state (a PostState; scene = state.make_scene()): graph B ends with the state's parameter step, whose xyz lr is
     state.set_learning_rate's.  An overflowed frame (binning or rows) changes no state; re-run it through
-    pipeline.post_step(state=).  capture()'s warm-up changes no state."""
+    pipeline.post_step(state=).  capture()'s warm-up changes no state.  cull: the view-culled cut (GraphedLodCut)."""
 
     def __init__(self, scene, W, H, tanfovx, tanfovy, bg, threshold, lambda_dssim=0.2, exposure=False, mask=False,
                  sh_degree=3, row_capacity=None, bin_capacity=1 << 22, sort_capacity=4096, world=1, capture=True,
-                 state=None):
+                 state=None, cull=False):
         if int(world) != 1:
             raise ValueError("GraphedPostStep runs on one GPU: the SSIM window reaches across the tile-row shards")
         if state is not None:
@@ -152,7 +152,7 @@ class GraphedPostStep(GraphedStep):
                 raise ValueError(f"SH degree {sh_degree} needs more than the state's {state.sh_coeffs} coefficients")
         self.state, self._update, self._pargs = state, state is not None, None
         super().__init__(scene, W, H, tanfovx, tanfovy, bg, threshold, sh_degree=sh_degree, row_capacity=row_capacity,
-                         bin_capacity=bin_capacity, sort_capacity=sort_capacity, capture=False)
+                         bin_capacity=bin_capacity, sort_capacity=sort_capacity, capture=False, cull=cull)
         self._init_post_loss(lambda_dssim, exposure, mask)
         self.status_dev = torch.zeros(8, dtype=torch.float64, device=self.dev)
         if capture:

@@ -242,6 +242,29 @@ int h3dgs_lod_budget(int32_t N, const int32_t* nodes, const float* boxes, const 
                      int32_t* info_out, void* scratch, void* stream);
 size_t h3dgs_lod_budget_scratch_bytes(int32_t N);
 
+/* View cull of the cut (csrc/lod_cull.cu; DESIGN.md §3.9): row_mask[r] [device uint8, one byte per Gaussian row] = 1
+ * for every row of every node that the rasterizer could draw for this camera -- a positive radius and a non-empty tile
+ * rect for some lerp weight t in [0, 1] with its partner row (the parent node's start row; the row itself for a root)
+ * --, 0 for the others; rows that belong to no node are not written.  A superset of what K1 draws, independent of the
+ * threshold, so one mask serves the cut and the budget at every threshold.  viewmatrix / projmatrix [device, 16 floats
+ * each] and W, H, tanfov, scale_modifier as the frame's h3dgs_raster_args; precomputed 3D covariances are not
+ * supported.  Capturable, no host synchronisation. */
+int h3dgs_lod_cull_mask(int32_t N, const int32_t* nodes, const float* means3D, const float* scales, const float* rotations,
+                        float scale_modifier, const float* viewmatrix, const float* projmatrix, int32_t W, int32_t H,
+                        float tanfovx, float tanfovy, uint8_t* row_mask, void* stream);
+
+/* h3dgs_lod_cut and h3dgs_lod_budget under a row mask (NULL: every row, the unmasked calls bit for bit): a node's count
+ * is the number of masked rows in its range, the cut emits only those, in order, with the fields they have without the
+ * mask, and the budget counts only those (the rows of the culled cut). */
+int h3dgs_lod_cut_masked(int32_t N, const int32_t* nodes, const float* boxes, float target_size,
+                         const float* target_size_dev, const float* viewpoint, const uint8_t* row_mask,
+                         int32_t* render_indices, int32_t* parent_indices, int32_t* nodes_for_render_indices,
+                         float* ts, int32_t* num_kids, int32_t* count, void* scratch, void* stream);
+int h3dgs_lod_budget_masked(int32_t N, const int32_t* nodes, const float* boxes, const float* viewpoint,
+                            const uint8_t* row_mask, float floor_size, const float* floor_dev, int32_t budget,
+                            const int32_t* budget_dev, float* threshold_out, int32_t* info_out, void* scratch,
+                            void* stream);
+
 /* ---- peer memory for the tile-sharded multi-GPU mode (csrc/peer.cu) ----
  * h3dgs_peer_alloc: zero-filled device allocation that can be exported to the other ranks' processes (CUDA IPC);
  * h3dgs_peer_export / h3dgs_peer_open: 64-byte handle out / mapped pointer in (the host side exchanges the handles,
@@ -696,6 +719,7 @@ enum {
     H3DGS_STAGE_GATHER, H3DGS_STAGE_RENDER_FWD, H3DGS_STAGE_RENDER_BWD, H3DGS_STAGE_PREPROCESS_BWD,
     H3DGS_STAGE_LOD_CUT, H3DGS_STAGE_LOD_WEIGHTS, H3DGS_STAGE_PREPROCESS_COLOR, H3DGS_STAGE_SH_BACKWARD,
     H3DGS_STAGE_LOSS_BACKWARD_EXPOSURE, H3DGS_STAGE_INVDEPTH_L1, H3DGS_STAGE_DENSIFY_STATS, H3DGS_STAGE_LOD_BUDGET,
+    H3DGS_STAGE_LOD_CULL,
     H3DGS_STAGE_COUNT
 };
 int h3dgs_profile_enable(int on);
