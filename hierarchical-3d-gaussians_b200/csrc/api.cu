@@ -105,6 +105,33 @@ int pinned_scratch(void** out) {
     return H3DGS_OK;
 }
 
+// ---- per device: the count of writers of each full-size dL/dSH row (launch_sh_row_count), for the SH backward's own-row
+// stores.  A captured graph keeps the pointer it was captured with, so a buffer is never freed: a larger one replaces it
+// outside capture only; a capture that finds it too small gets none, and its SH backward reduces every row.  Calls on one
+// device share it as they share the side stream: two backward graphs replayed at once on one device would race on it ----
+struct RowCounts { int* p = nullptr; size_t n = 0; };
+static RowCounts g_row_counts[64];
+static int row_counts(size_t n, cudaStream_t s, int** out) {
+    *out = nullptr;
+    int dev = 0;
+    H3_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64) { set_error("device index %d out of range", dev); return H3DGS_EINVAL; }
+    RowCounts& rc = g_row_counts[dev];
+    if (rc.n < n) {
+        if (capturing(s)) return H3DGS_OK;
+        void* p = nullptr;
+#ifdef H3_SIMT_EMU
+        p = malloc(n * sizeof(int));
+        if (!p) { set_error("row count buffer: out of memory"); return H3DGS_ENOMEM; }
+#else
+        H3_CUDA(cudaMalloc(&p, n * sizeof(int)));
+#endif
+        rc.p = static_cast<int*>(p); rc.n = n;
+    }
+    *out = rc.p;
+    return H3DGS_OK;
+}
+
 // rows read as float4: rotations (preprocess_kernel, preprocess_backward_kernel) and shs when 3 M is a multiple of 4
 // (the SH kernels); a contiguous view at an odd float offset would be read misaligned
 static bool misaligned16(const void* p, const char* who) {
@@ -331,6 +358,10 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
     const bool fill_now = a->render_indices && (((phases & 2) && !(phases & 8)) || (phases & 4));
     const bool sh_fill_in_replay = fill_now && (phases & 1) && D > 0;
     const size_t sh_floats = (size_t)a->num_source * a->sh_coeffs * 3;
+    // the SH backward runs on the side stream, after the fill, in this call (below): it may store the rows it alone
+    // writes, counted here beside the replay
+    const bool side_k9 = fill_now && (phases & 2) && !a->debug && !a->colors_precomp;
+    int* row_count = nullptr;
     if (fill_now) {
         rc = side_stream(&ss);
         if (rc) return rc;
@@ -343,6 +374,14 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
         if (!sh_fill_in_replay) H3_CUDA(cudaMemsetAsync(dL_dsh, 0, sh_floats * sizeof(float), ss->s));
         H3_CUDA(cudaMemsetAsync(dL_dscales, 0, N * 3 * sizeof(float), ss->s));
         H3_CUDA(cudaMemsetAsync(dL_drotations, 0, N * 4 * sizeof(float), ss->s));
+        if (side_k9 && ((a->sh_coeffs * 3) & 3) == 0) {
+            rc = row_counts(N, ss->s, &row_count);
+            if (rc) return rc;
+            if (row_count) {
+                rc = launch_sh_row_count(*a, row_count, ss->s);
+                if (rc) return rc;
+            }
+        }
         H3_CUDA(cudaEventRecord(ss->join, ss->s));
         zero_joined = false;
     }
@@ -361,11 +400,12 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
     }
     if (!(phases & 2)) return H3DGS_OK;
     if (!zero_joined && !a->debug && !a->colors_precomp) {
-        // scatter mode: every output is an atomic reduction, so the SH kernel (side stream, after the
-        // fill) and the covariance kernel (main stream) run concurrently
+        // scatter mode: every output is an atomic reduction or a row no other kernel writes, so the SH kernel (side
+        // stream, after the fill) and the covariance kernel (main stream) run concurrently
         H3_CUDA(cudaEventRecord(ss->fork, s));                           // accum is complete at this point of s
         H3_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
-        rc = launch_sh_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, dL_dmeans3D, dL_dsh, ss->s);
+        rc = launch_sh_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, row_count, dL_dmeans3D,
+                                dL_dsh, ss->s);
         if (rc) return rc;
         H3_CUDA(cudaStreamWaitEvent(s, ss->join, 0));                    // zero-fill done before our own reductions
         H3_CUDA(cudaEventRecord(ss->join, ss->s));
@@ -379,7 +419,8 @@ extern "C" int h3dgs_rasterize_backward(const h3dgs_raster_args* a, const int32_
     rc = launch_preprocess_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, dL_dmeans3D, dL_dmeans2D,
                                     dL_dsh, dL_dcolors_precomp, dL_dopacities, dL_dscales, dL_drotations, dL_dcov3D, s);
     if (rc) return rc;
-    return launch_sh_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, dL_dmeans3D, dL_dsh, s);
+    return launch_sh_backward(b, radii, geom + gl.rank_mask, (const Record*)(geom + gl.records), accum, nullptr, dL_dmeans3D,
+                              dL_dsh, s);
 }
 
 extern "C" int h3dgs_state_layout(int32_t P, int32_t W, int32_t H, int64_t D, const void* geom_state,

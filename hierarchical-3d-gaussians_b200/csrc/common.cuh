@@ -140,7 +140,8 @@ int launch_tile_binning(const h3dgs_raster_args& a, const int32_t* radii, const 
 int launch_preprocess_color(const h3dgs_raster_args& a, const int32_t* radii, const uint32_t* tiles_touched,
                             Record* records, cudaStream_t s);
 int launch_sh_backward(const h3dgs_raster_args& a, const int32_t* radii, const uint8_t* rank_mask, const Record* records,
-                       const float* accum, float* dL_dmeans3D, float* dL_dsh, cudaStream_t s);
+                       const float* accum, const int* row_count, float* dL_dmeans3D, float* dL_dsh, cudaStream_t s);
+int launch_sh_row_count(const h3dgs_raster_args& a, int* count, cudaStream_t s);
 int launch_scan(const uint32_t* in, uint32_t* out, int n, void* temp, size_t temp_bytes, cudaStream_t s, bool debug);
 size_t scan_temp_bytes(int n);
 size_t sort_temp_bytes(int64_t n);
