@@ -161,33 +161,6 @@ int launch_preprocess_backward(const h3dgs_raster_args& a, const int32_t* radii,
                                float* dL_dcolors, float* dL_dopacities, float* dL_dscales, float* dL_drots,
                                float* dL_dcov3D, cudaStream_t s);
 
-#ifdef __CUDACC__
-// Pixel layout of the blend kernels: CTA = 128 threads = 4 warps; warp q owns the 8x8 quadrant
-// (q & 1, q >> 1) of the 16x16 tile; lane l owns column (l & 7) and the two rows 2*(l >> 3), +1.
-__device__ __forceinline__ void quad_pixel(int tile_x, int tile_y, int warp, int lane, int& px, int& py0) {
-    px = tile_x * kTile + 8 * (warp & 1) + (lane & 7);
-    py0 = tile_y * kTile + 8 * (warp >> 1) + 2 * (lane >> 3);
-}
-
-// Group walk (render_*_kernel<..., GROUPS = true>): the same quadrant per warp, but lanes 8 g .. 8 g + 7 own the
-// 4x4-pixel block g = (g & 1, g >> 1) of it -- lane k of the group: column (k & 3), rows 2 (k >> 2), +1 -- and each
-// 8-lane group walks only the entries whose block bit is set (common.cuh kBlockShift, binning.cu::block_mask16).
-__device__ __forceinline__ void group_pixel(int tile_x, int tile_y, int warp, int lane, int& px, int& py0) {
-    const int g = lane >> 3, k = lane & 7;
-    px = tile_x * kTile + 8 * (warp & 1) + 4 * (g & 1) + (k & 3);
-    py0 = tile_y * kTile + 8 * (warp >> 1) + 4 * (g >> 1) + 2 * (k >> 2);
-}
-// Each kernel defaults to the walk that is faster for it on the H100 (DESIGN.md §3.1): the backward walks per group (on
-// config #3 it runs 27 % fewer loop iterations than the one-list-per-warp walk, at 2.3x the gradient reductions), the
-// forward walks one list per warp.  H3DGS_GROUPWALK=1 forces the group walk in both kernels, H3DGS_GROUPWALK=0 one list per warp in both; the two walks
-// compute the same results bit for bit.
-inline bool use_group_walk(bool dflt) {
-    const char* e = getenv("H3DGS_GROUPWALK");
-    return (e && e[0]) ? e[0] != '0' : dflt;
-}
-
-#endif
-
 // peer mode (h3dgs_raster_args.peer_count > 1): device pointers into the memory of every rank, by value in the kernel parameters
 struct PeerPtrs { void* p[H3DGS_MAX_PEERS]; int n; };
 inline PeerPtrs peer_ptrs(void* const* src, int n) {
@@ -250,7 +223,7 @@ int launch_peer_push(const h3dgs_raster_args& a, const uint8_t* rank_mask, const
 
 // Loop statistics of the blend kernels, HOST EMULATION BUILD ONLY (tests/emul; the emulator is single-threaded):
 // 0 bwd warp iterations | 1 bwd iterations left at the no-taker vote | 2 bwd pixel-entries taken | 3 bwd group-iterations
-// with an entry | 4 of those without any taker | 8 fwd warp iterations | 9 fwd pixel-entries taken | 10 fwd group-iterations
+// with an entry | 4 of those without any taker | 8 fwd warp iterations | 9 fwd pixel-entries taken
 #ifdef H3_SIMT_EMU
 extern long long g_emu_stats[16];
 #define H3_STAT(i, n) (h3dgs::g_emu_stats[i] += (n))

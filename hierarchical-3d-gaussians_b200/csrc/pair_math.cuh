@@ -143,13 +143,12 @@ H3_PM_FN void pair_hier_alpha(f2 a, float t, uint32_t k /* num_node_kids */, f2&
 // T: transmittance in front of the entry.  Returns the blend weights w = alpha T (0 for a pixel that
 // does not take the entry), updates T, and reports per pixel whether it took the entry (v) and
 // whether it terminated on it (done: T (1 - alpha) < 1e-4; the entry is then NOT blended).
-// active = false: this lane has no entry in this iteration (group walk); nothing is taken, nothing terminates.
-H3_PM_FN f2 pair_blend(f2 pw, f2 al, f2& T, bool& done0, bool& done1, bool& v0, bool& v1, bool active = true) {
+H3_PM_FN f2 pair_blend(f2 pw, f2 al, f2& T, bool& done0, bool& done1, bool& v0, bool& v1) {
     const f2 tT = mul2(T, sub2(bc(1.0f), al));
     float pw0, pw1, al0, al1, tT0, tT1;
     upk(pw, pw0, pw1); upk(al, al0, al1); upk(tT, tT0, tT1);
-    v0 = active && !done0 && pw0 <= 0.0f && al0 >= kAlphaSkip;
-    v1 = active && !done1 && pw1 <= 0.0f && al1 >= kAlphaSkip;
+    v0 = !done0 && pw0 <= 0.0f && al0 >= kAlphaSkip;
+    v1 = !done1 && pw1 <= 0.0f && al1 >= kAlphaSkip;
     if (v0 && tT0 < kTStop) { done0 = true; v0 = false; }
     if (v1 && tT1 < kTStop) { done1 = true; v1 = false; }
     const f2 w = sel2(v0, v1, mul2(al, T), bc(0.f));

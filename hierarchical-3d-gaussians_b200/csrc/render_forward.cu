@@ -13,22 +13,23 @@
 
 namespace h3dgs {
 
-#ifdef H3_BLEND_OCC8      /* see render_backward.cu */
-constexpr int kFwdBatch = 224;
-constexpr int kFwdMinBlocks = 8;
-#else
 constexpr int kFwdBatch = 256;
 constexpr int kFwdMinBlocks = 1;
-#endif
 constexpr int kFwdStages = 2;
 
 // Two vertically adjacent pixels per thread: CTA = 128 threads = 4 warps, warp q owns one 8x8-pixel
-// quadrant of the tile (common.cuh::quad_pixel).
-// The entry's record, its dx terms, the survivor loop and (in backward) the warp reduction are
+// quadrant of the tile (quad_pixel).
+// The entry's record, its dx terms, the survivor loop and (in backward) the 8-lane reduction are
 // shared by the two pixels; only the per-pixel arithmetic of the pair (pair_math.cuh) is done twice.
 constexpr int kFwdThreads = 128;
 
-template <bool HIER, bool DEPTH, bool GROUPS>
+// warp q's quadrant is (q & 1, q >> 1); lane l owns its column (l & 7) and the two rows 2*(l >> 3), +1
+__device__ __forceinline__ void quad_pixel(int tile_x, int tile_y, int warp, int lane, int& px, int& py0) {
+    px = tile_x * kTile + 8 * (warp & 1) + (lane & 7);
+    py0 = tile_y * kTile + 8 * (warp >> 1) + 2 * (lane >> 3);
+}
+
+template <bool HIER, bool DEPTH>
 __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks)
 render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, const uint2* __restrict__ ranges,
                       const Record* __restrict__ sorted, const float* __restrict__ bg, float* __restrict__ out_color,
@@ -38,7 +39,6 @@ render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, co
     __shared__ __align__(128) Record s_rec[kFwdStages][kFwdBatch];
     __shared__ __align__(8) uint64_t s_full[kFwdStages];
     __shared__ uint32_t s_max;
-    __shared__ uint8_t s_list[GROUPS ? kFwdThreads / 32 : 1][4][GROUPS ? kFwdBatch : 4];   // group walk: per warp, four lists of entry positions
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile_x = blockIdx.x % gx;
@@ -66,8 +66,7 @@ render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, co
     issued = min(kFwdStages, nb);
 
     int px, py0;
-    if (GROUPS) group_pixel(tile_x, tile_y, warp, lane, px, py0);
-    else quad_pixel(tile_x, tile_y, warp, lane, px, py0);
+    quad_pixel(tile_x, tile_y, warp, lane, px, py0);
     const int py1 = py0 + 1;
     const bool in0 = px < W && py0 < H, in1 = px < W && py1 < H;
     const float fpx = (float)px;
@@ -78,7 +77,6 @@ render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, co
     float Ca0 = 0.f, Ca1 = 0.f, Ca2 = 0.f, Cb0 = 0.f, Cb1 = 0.f, Cb2 = 0.f, inv0 = 0.f, inv1 = 0.f;
     uint32_t last0 = 0, last1 = 0;
     const int qsel = kBlockShift + 4 * warp;                // this warp's four block bits in the entries' reach mask
-    const int grp = lane >> 3;
 
     int waited = 0;
     for (int b = 0; b < nb; b++) {
@@ -89,9 +87,8 @@ render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, co
         const Record* rec = &s_rec[st][0];
         const uint32_t base = (uint32_t)(b * kFwdBatch);
         // one entry at the thread's two pixels (straight-line: a per-thread `continue`/`break` here leaves the warp split
-        // into fragments that each re-walk the list -- measured: 18x the instructions); has = false: this lane's group
-        // has no entry in this iteration, nothing is taken
-        auto blend_entry = [&](int j, bool has) {
+        // into fragments that each re-walk the list -- measured: 18x the instructions)
+        auto blend_entry = [&](int j) {
             const float4 a = rec[j].a;
             const float4 bb = rec[j].b;
             const float4 c = rec[j].c;
@@ -101,66 +98,28 @@ render_forward_kernel(int W, int H, int gx, int shard_count, int shard_index, co
             pair_gauss(pw, bb.y, G, al);
             pair_hier_alpha<HIER, false>(al, bb.z, kb & kSortedKidsMask, al, unused);
             bool v0, v1;
-            const f2 w = pair_blend(pw, al, T, done0, done1, v0, v1, has);
+            const f2 w = pair_blend(pw, al, T, done0, done1, v0, v1);
             upk(fma2(bc(c.x), w, pk(Ca0, Cb0)), Ca0, Cb0);
             upk(fma2(bc(c.y), w, pk(Ca1, Cb1)), Ca1, Cb1);
             upk(fma2(bc(c.z), w, pk(Ca2, Cb2)), Ca2, Cb2);
             if (DEPTH) upk(fma2(bc(c.w), w, pk(inv0, inv1)), inv0, inv1);
             if (lane == 0) H3_STAT(8, 1);
-            if ((lane & 7) == 0 && has) H3_STAT(10, 1);
             H3_STAT(9, (v0 ? 1 : 0) + (v1 ? 1 : 0));
             const uint32_t idx = base + (uint32_t)j + 1u;
             last0 = v0 ? idx : last0; last1 = v1 ? idx : last1;
         };
-        if (GROUPS) {
-            // Group walk.  Each 8-lane group owns a 4x4 block and blends only the entries whose block bit is set.  Per BATCH
-            // the warp compacts four lists of entry positions in shared memory (per round of 32 entries: one mask test per
-            // lane, four ballots, four predicated byte stores); the four groups then advance in lockstep, each through its
-            // own list, for max(len) iterations -- balancing the groups over 256 entries instead of 32.
-            uint8_t* lst = &s_list[warp][0][0];
-            const uint32_t dm = __ballot_sync(0xffffffffu, done0 && done1);
-            if (dm != 0xffffffffu) {
-                // groups whose 16 pixels are finished list nothing
-                const uint32_t live = ((dm & 0xFFu) != 0xFFu ? 1u : 0u) | (((dm >> 8) & 0xFFu) != 0xFFu ? 2u : 0u) |
-                                      (((dm >> 16) & 0xFFu) != 0xFFu ? 4u : 0u) | ((dm >> 24) != 0xFFu ? 8u : 0u);
-                const uint32_t lt = (1u << lane) - 1u;
-                int c0 = 0, c1 = 0, c2 = 0, c3 = 0;
-                for (int j0 = 0; j0 < cnt; j0 += 32) {
-                    const int jl = j0 + lane;
-                    const uint32_t nib = jl < cnt ? (__float_as_uint(rec[jl].b.w) >> qsel) & live : 0u;
-                    const uint32_t m0 = __ballot_sync(0xffffffffu, nib & 1u), m1 = __ballot_sync(0xffffffffu, nib & 2u);
-                    const uint32_t m2 = __ballot_sync(0xffffffffu, nib & 4u), m3 = __ballot_sync(0xffffffffu, nib & 8u);
-                    if (nib & 1u) lst[c0 + __popc(m0 & lt)] = (uint8_t)jl;
-                    if (nib & 2u) lst[kFwdBatch + c1 + __popc(m1 & lt)] = (uint8_t)jl;
-                    if (nib & 4u) lst[2 * kFwdBatch + c2 + __popc(m2 & lt)] = (uint8_t)jl;
-                    if (nib & 8u) lst[3 * kFwdBatch + c3 + __popc(m3 & lt)] = (uint8_t)jl;
-                    c0 += __popc(m0); c1 += __popc(m1); c2 += __popc(m2); c3 += __popc(m3);
-                }
-                __syncwarp();
-                const int mylen = grp == 0 ? c0 : grp == 1 ? c1 : grp == 2 ? c2 : c3;
-                const int maxlen = max(max(c0, c1), max(c2, c3));
-                const uint8_t* my = lst + grp * kFwdBatch;
-                for (int i = 0; i < maxlen; i++) {
-                    const bool has = i < mylen;
-                    blend_entry(has ? (int)my[i] : 0, has);
-                    if ((i & 15) == 15 && __all_sync(0xffffffffu, done0 && done1)) break;
-                }
-                __syncwarp();                 // the lists are rebuilt for the next batch
-            }
-        } else {
-            // One list per warp: per round of 32 entries each lane tests ONE entry against this warp's quadrant and a ballot
-            // compacts the survivors, so culled entries cost nothing per pixel.  The survivor loop is warp-uniform (same
-            // mask in every lane).  A warp leaves the batch only when all of its 64 pixels are done.
-            for (int j0 = 0; j0 < cnt; j0 += 32) {
-                if (__all_sync(0xffffffffu, done0 && done1)) break;
-                const int jl = j0 + lane;
-                const uint32_t nib = jl < cnt ? (__float_as_uint(rec[jl].b.w) >> qsel) & 0xFu : 0u;
-                uint32_t m = __ballot_sync(0xffffffffu, nib != 0u);
-                while (m != 0u) {
-                    const int j = j0 + __ffs(m) - 1;
-                    m &= m - 1;
-                    blend_entry(j, true);
-                }
+        // One list per warp: per round of 32 entries each lane tests ONE entry against this warp's quadrant and a ballot
+        // compacts the survivors, so culled entries cost nothing per pixel.  The survivor loop is warp-uniform (same
+        // mask in every lane).  A warp leaves the batch only when all of its 64 pixels are done.
+        for (int j0 = 0; j0 < cnt; j0 += 32) {
+            if (__all_sync(0xffffffffu, done0 && done1)) break;
+            const int jl = j0 + lane;
+            const uint32_t nib = jl < cnt ? (__float_as_uint(rec[jl].b.w) >> qsel) & 0xFu : 0u;
+            uint32_t m = __ballot_sync(0xffffffffu, nib != 0u);
+            while (m != 0u) {
+                const int j = j0 + __ffs(m) - 1;
+                m &= m - 1;
+                blend_entry(j);
             }
         }
         const int ndone = __syncthreads_count(done0 && done1);
@@ -232,16 +191,13 @@ int launch_render_forward(const h3dgs_raster_args& a, const uint32_t* ranges, co
     const bool depth = a.do_depth != 0;
     const dim3 grid(gx * rows), block(kFwdThreads);
     ProfScope prof(H3DGS_STAGE_RENDER_FWD, s);
-    const bool groups = use_group_walk(false);
     const PeerPtrs peers = peer_ptrs(a.peer_image, a.peer_count);
-#define LAUNCH(HI, DE, GR)                                                                                         \
-    render_forward_kernel<HI, DE, GR><<<grid, block, 0, s>>>(W, H, gx, sc, si, (const uint2*)ranges, sorted_records, \
-                                                             a.bg, out_color, out_invdepth, final_T, n_contrib,      \
-                                                             tile_max_contrib, peers)
-#define LAUNCH2(HI, DE) do { if (groups) LAUNCH(HI, DE, true); else LAUNCH(HI, DE, false); } while (0)
-    if (hier) { if (depth) LAUNCH2(true, true); else LAUNCH2(true, false); }
-    else      { if (depth) LAUNCH2(false, true); else LAUNCH2(false, false); }
-#undef LAUNCH2
+#define LAUNCH(HI, DE)                                                                                         \
+    render_forward_kernel<HI, DE><<<grid, block, 0, s>>>(W, H, gx, sc, si, (const uint2*)ranges, sorted_records, \
+                                                         a.bg, out_color, out_invdepth, final_T, n_contrib,      \
+                                                         tile_max_contrib, peers)
+    if (hier) { if (depth) LAUNCH(true, true); else LAUNCH(true, false); }
+    else      { if (depth) LAUNCH(false, true); else LAUNCH(false, false); }
 #undef LAUNCH
     H3_LAUNCHED("render_forward", a.debug, s);
     return H3DGS_OK;

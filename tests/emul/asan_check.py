@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.  A memcheck for the kernels without a GPU: build the emulation library with
 AddressSanitizer (heap and globals -- `__shared__` arrays are globals in the emulator; stack instrumentation is off
 because the fibers switch stacks by hand), preload libasan so that numpy's buffers get red zones too, and run a set
-of scenes through both blend variants, the sharded schedule, the fused cut gather, the device-side LOD cut /
+of scenes through the blend kernels, the sharded schedule, the fused cut gather, the device-side LOD cut /
 capacity mode, and the preprocess edge families with non-finite inputs and huge splats (tests/preprocess_ref.py).  Usage:   python tests/emul/asan_check.py          (re-executes itself under LD_PRELOAD)
 A deliberately short output buffer is reported as heap-buffer-overflow (checked by --negative-control)."""
 import os
@@ -65,22 +65,20 @@ def run_cases(so, negative):
     TP.hold(emu, PR.family_degenerate())
     n += 2
     print(f"asan: {n} non-finite / huge / degenerate cases done", flush=True)
-    for gw in ("0", "1"):
-        os.environ["H3DGS_GROUPWALK"] = gw
-        for (P, W, H, kw, depth) in [(3000, 256, 192, dict(mode="hier", seed=42), True), (1500, 160, 96, dict(seed=7), False),
-                                     (300, 15, 33, dict(seed=3, scale_k=2e-2), False),
-                                     (6000, 96, 64, dict(seed=11, scale_k=3e-2, zmax=6.0), False),
-                                     (16000, 48, 48, dict(seed=13, scale_k=6e-2, zmax=4.0), False)]:
-            cam, sc, ts, kids, bg = make_scene(P, W, H, **kw)
-            T._check(emu, cam, sc, bg, ts, kids, do_depth=depth, tol=5e-5)
-            n += 1
-        for t in (T.test_tile_shards_equal_the_whole_frame, T.test_sharded_frame_with_row_blocks,
-                  T.test_fused_cut_gather_and_scatter, T.test_device_lod_cut_and_skipped_rows):
-            t(emu)
-            n += 1
-        for G in (2, 4):                                   # peer mode: rank mask, push into the staging areas, gather in K9
-            T.test_peer_mode_fused_collectives_schedule(emu, G)
-            n += 1
+    for (P, W, H, kw, depth) in [(3000, 256, 192, dict(mode="hier", seed=42), True), (1500, 160, 96, dict(seed=7), False),
+                                 (300, 15, 33, dict(seed=3, scale_k=2e-2), False),
+                                 (6000, 96, 64, dict(seed=11, scale_k=3e-2, zmax=6.0), False),
+                                 (16000, 48, 48, dict(seed=13, scale_k=6e-2, zmax=4.0), False)]:
+        cam, sc, ts, kids, bg = make_scene(P, W, H, **kw)
+        T._check(emu, cam, sc, bg, ts, kids, do_depth=depth, tol=5e-5)
+        n += 1
+    for t in (T.test_tile_shards_equal_the_whole_frame, T.test_sharded_frame_with_row_blocks,
+              T.test_fused_cut_gather_and_scatter, T.test_device_lod_cut_and_skipped_rows):
+        t(emu)
+        n += 1
+    for G in (2, 4):                                   # peer mode: rank mask, push into the staging areas, gather in K9
+        T.test_peer_mode_fused_collectives_schedule(emu, G)
+        n += 1
     # round 2: the in-register tile sort over all size classes, the TMA-staged single-pass cut (bulk and plain-load paths),
     # the L1 kernel's image forwarding, the split-phase zero-fill
     T.test_register_sort_size_classes_with_equal_depths(emu)

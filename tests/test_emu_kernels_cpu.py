@@ -39,18 +39,10 @@ def grad_close(a, b, name, tol=1e-5, max_rows=12):
 
 
 @pytest.fixture(scope="module")
-def emu_lib(tmp_path_factory):
+def emu(tmp_path_factory):
     from build_emu import build
     from emu_api import Emu
     return Emu(build(str(tmp_path_factory.mktemp("h3dgs_emu"))))
-
-
-@pytest.fixture(params=["quadrants", "groups"])
-def emu(emu_lib, request, monkeypatch):
-    """both variants of the blend kernels: one survivor list per warp (8x8 quadrant), or one per 8-lane group
-    (4x4 block; H3DGS_GROUPWALK=1)"""
-    monkeypatch.setenv("H3DGS_GROUPWALK", "1" if request.param == "groups" else "0")
-    return emu_lib
 
 
 def _check(emu, cam, sc, bg, ts=None, kids=None, do_depth=False, sh_degree=3, colors=None, cov=None, tol=1e-5):
@@ -254,7 +246,7 @@ def test_equal_depths_and_long_lists_fall_back_to_the_global_sort(emu):
     assert (st["ranges"][:, 1] - st["ranges"][:, 0]).max() > 8192    # longer than the shared-memory sort handles
 
 
-def test_register_sort_size_classes_with_equal_depths(emu_lib):
+def test_register_sort_size_classes_with_equal_depths(emu):
     """tile lists of 33 .. ~700 entries: every size class of the in-register sort (1, 2, 4, 8 keys per thread), with
     many equal depths, so the (depth bits, index) order -- the stable order of the reference's global sort -- is
     checked through the lane exchanges, the in-thread stages and the cross-warp stages alike"""
@@ -268,9 +260,9 @@ def test_register_sort_size_classes_with_equal_depths(emu_lib):
     f = oracle_run(cam, sc, bg, backward=False)[0]
     lens = f["ranges"].reshape(-1, 2)[:, 1] - f["ranges"].reshape(-1, 2)[:, 0]
     assert all(((lens > lo) & (lens <= hi)).any() for lo, hi in [(0, 128), (128, 256), (256, 512), (512, 1024)])
-    a, keepalive = emu_lib.args(cam, bg, sc)
-    fw = emu_lib.forward(a, keepalive)
-    st = emu_lib.state(a, fw)
+    a, keepalive = emu.args(cam, bg, sc)
+    fw = emu.forward(a, keepalive)
+    st = emu.state(a, fw)
     assert fw["D"] == f["num_rendered"]
     assert np.array_equal(st["keys_sorted"], f["keys"])
     assert np.array_equal(st["point_list"], f["point_list"])
@@ -324,7 +316,7 @@ def test_fused_l1_loss_and_gradient(emu, W, shard):
     assert np.all(out[:, ~own] == 7.0)
 
 
-def test_split_phases_fill_the_scatter_outputs_beside_the_replay(emu_lib):
+def test_split_phases_fill_the_scatter_outputs_beside_the_replay(emu):
     """scatter mode, backward in two calls: phases 1|4 (replay + zero-fill of the full-size gradients) then 2|8 (chain rule,
     outputs already zero) gives what the single call (3) gives; the outputs are poisoned first, so a missing fill shows."""
     from oracle import oracle
@@ -337,26 +329,26 @@ def test_split_phases_fill_the_scatter_outputs_beside_the_replay(emu_lib):
     n, ri, pi, ni = oracle.expand_to_size(h["nodes"], h["boxes"], thr, cam.camera_center)
     ts, kids = oracle.get_interpolation_weights(ni, thr, h["nodes"], h["boxes"], cam.camera_center)
     bg = np.array([0.3, 0.2, 0.1], np.float32)
-    a, keep = emu_lib.args(cam, bg, h, ts=ts, kids=kids, ridx=ri, pidx=pi)
-    fw = emu_lib.forward(a, keep)
+    a, keep = emu.args(cam, bg, h, ts=ts, kids=kids, ridx=ri, pidx=pi)
+    fw = emu.forward(a, keep)
     gcol = synth.l1_grad(fw["color"])
-    whole = emu_lib.backward(a, fw, gcol)
-    first = emu_lib.backward(a, fw, gcol, phases=1 | 4)
+    whole = emu.backward(a, fw, gcol)
+    first = emu.backward(a, fw, gcol, phases=1 | 4)
     assert all(not np.asarray(first[k]).any() for k in ("means3D", "sh", "opacities", "scales", "rotations"))
     for k in ("means3D", "sh", "opacities", "scales", "rotations"):
         first[k][...] += 0.0                                     # the arrays the second call continues with
-    second = emu_lib.backward(a, fw, gcol, phases=2 | 8, scratch=first["scratch"], outs=first)
+    second = emu.backward(a, fw, gcol, phases=2 | 8, scratch=first["scratch"], outs=first)
     for k in ("means3D", "sh", "opacities", "scales", "rotations", "means2D"):
         assert np.allclose(second[k], whole[k], rtol=1e-5, atol=1e-9), k
     # without the fill flag of the first call and with "already zero" claimed, stale contents would survive: the fill matters
     stale = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in first.items()}
     stale["means3D"][...] = 3.0
-    third = emu_lib.backward(a, fw, gcol, phases=2 | 8, scratch=first["scratch"], outs=stale)
+    third = emu.backward(a, fw, gcol, phases=2 | 8, scratch=first["scratch"], outs=stale)
     assert not np.allclose(third["means3D"], whole["means3D"])
 
 
 @pytest.mark.parametrize("G", [2, 4])
-def test_peer_l1_kernel_forwards_the_rendered_rows(emu_lib, G):
+def test_peer_l1_kernel_forwards_the_rendered_rows(emu, G):
     """h3dgs_l1_loss_grad_peer with peer_images: every "rank" holds only ITS tile rows of the frame; its L1 pass copies
     them into the images of the other ranks (the fused all-gather of the peer-mode step) while it evaluates the loss of
     those rows -- afterwards every image is the whole frame, every loss sum the loss of the whole frame."""
@@ -377,8 +369,8 @@ def test_peer_l1_kernel_forwards_the_rendered_rows(emu_lib, G):
     for r in range(G):
         ls = (C.c_void_p * G)(*[s_.ctypes.data for s_ in sums])
         ims = (C.c_void_p * G)(*[im.ctypes.data for im in images])
-        rc = emu_lib.L.h3dgs_l1_loss_grad_peer(3, H, W, p(images[r]), p(gt), C.c_float(0.5), G, r, p(outs[r]), G, ls, ims, None)
-        assert rc == 0, emu_lib.L.h3dgs_last_error()
+        rc = emu.L.h3dgs_l1_loss_grad_peer(3, H, W, p(images[r]), p(gt), C.c_float(0.5), G, r, p(outs[r]), G, ls, ims, None)
+        assert rc == 0, emu.L.h3dgs_last_error()
     for r in range(G):
         assert np.array_equal(images[r], frame)
         assert abs(sums[r][0] - np.abs((frame - gt).astype(np.float64)).sum()) < 1e-2
@@ -452,7 +444,7 @@ def test_peer_mode_fused_collectives_schedule(emu, G):
 
 @pytest.mark.parametrize("tau,misalign,agg_only", [(0.0, False, False), (6.0, False, False), (60.0, False, False), (6.0, True, False),
                                                    (6.0, False, True)])
-def test_single_pass_cut_over_many_tiles(emu_lib, tau, misalign, agg_only, monkeypatch):
+def test_single_pass_cut_over_many_tiles(emu, tau, misalign, agg_only, monkeypatch):
     """lod_cut_fused_kernel with 600+ tiles of 1024 nodes; indices, parents, nodes, weights (bit-exact) and kids against the
     oracle.  agg_only: the emulator runs the CTAs one after the other, so every predecessor would already show its inclusive
     prefix; the switch keeps all tiles but every 300th at "aggregate only", and the look-back has to add up to 299
@@ -471,7 +463,7 @@ def test_single_pass_cut_over_many_tiles(emu_lib, tau, misalign, agg_only, monke
     thr = synth.tau_threshold(tau, cam)
     n, ri, pi, ni = oracle.expand_to_size(h["nodes"], h["boxes"], thr, cam.camera_center)
     ts, kids = oracle.get_interpolation_weights(ni, thr, h["nodes"], h["boxes"], cam.camera_center)
-    L = emu_lib.L
+    L = emu.L
     nodes, boxes, vp = i32(h["nodes"]), f32(h["boxes"]), f32(cam.camera_center)
     assert nodes.ctypes.data % 16 == 0 and boxes.ctypes.data % 16 == 0        # whole tiles arrive by bulk copy (TMA wrappers) ...
     if misalign:                                                              # ... views that are not 16-B aligned by plain loads
@@ -484,7 +476,7 @@ def test_single_pass_cut_over_many_tiles(emu_lib, tau, misalign, agg_only, monke
     t2 = aligned(N * 4, np.float32, (N,))
     count = aligned(4, np.int32, (1,))
     scratch = aligned(L.h3dgs_expand_scratch_bytes(N))
-    emu_lib.check(L.h3dgs_lod_cut(N, ptr(nodes), ptr(boxes), thr, None, ptr(vp), ptr(r2), ptr(p2), ptr(n2), ptr(t2), ptr(k2),
+    emu.check(L.h3dgs_lod_cut(N, ptr(nodes), ptr(boxes), thr, None, ptr(vp), ptr(r2), ptr(p2), ptr(n2), ptr(t2), ptr(k2),
                                   ptr(count), ptr(scratch), None))
     assert int(count[0]) == n > 0
     assert np.array_equal(r2[:n], ri) and np.array_equal(p2[:n], pi) and np.array_equal(n2[:n], ni)
@@ -492,30 +484,30 @@ def test_single_pass_cut_over_many_tiles(emu_lib, tau, misalign, agg_only, monke
     assert (r2[n:] == -1).all()
 
 
-def test_prefiltered_flag_traps_on_a_culled_point(emu_lib):
+def test_prefiltered_flag_traps_on_a_culled_point(emu):
     """prefiltered=True is the caller's promise that nothing lies behind the near plane; the reference's kernel traps
     when the promise is broken -- here the forward returns an error instead of rendering."""
     cam, sc, ts, kids, bg = make_scene(300, 64, 48, seed=5)
-    a, keep = emu_lib.args(cam, bg, sc)
+    a, keep = emu.args(cam, bg, sc)
     a.prefiltered = 1
-    fw = emu_lib.forward(a, keep)                     # every point of this scene is in front of the camera
+    fw = emu.forward(a, keep)                     # every point of this scene is in front of the camera
     assert fw["D"] > 0
     sc2 = dict(sc); sc2["means3D"] = sc["means3D"].copy(); sc2["means3D"][7, 2] = -1.0
-    a2, keep2 = emu_lib.args(cam, bg, sc2)
+    a2, keep2 = emu.args(cam, bg, sc2)
     a2.prefiltered = 1
     with pytest.raises(RuntimeError, match="filtered although prefiltered"):
-        emu_lib.forward(a2, keep2)
+        emu.forward(a2, keep2)
     a2.prefiltered = 0
-    assert emu_lib.forward(a2, keep2)["radii"][7] == 0
+    assert emu.forward(a2, keep2)["radii"][7] == 0
 
 
-def test_tile_scan_over_more_than_one_pass(emu_lib):
+def test_tile_scan_over_more_than_one_pass(emu):
     """9000 tiles: the single-CTA tile scan needs two passes of 1024 x 8 tiles; ranges and keys against the oracle."""
     cam, sc, ts, kids, bg = make_scene(400, 1600, 1440, seed=13)
     f, b, gcol, gdep = oracle_run(cam, sc, bg, backward=False)
-    a, keep = emu_lib.args(cam, bg, sc)
-    fw = emu_lib.forward(a, keep)
-    st = emu_lib.state(a, fw)
+    a, keep = emu.args(cam, bg, sc)
+    fw = emu.forward(a, keep)
+    st = emu.state(a, fw)
     assert fw["D"] == f["num_rendered"] > 0
     assert np.array_equal(st["ranges"], f["ranges"]) and np.array_equal(st["keys_sorted"], f["keys"])
     assert np.array_equal(st["point_list"], f["point_list"])

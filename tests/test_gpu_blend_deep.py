@@ -1,6 +1,6 @@
 """GPU: the blend kernels (render_forward.cu, render_backward.cu) and the tile sort (binning.cu, api.cu) on DEEP tile
 lists, per pixel and per Gaussian against tests/blend_ref.py's float64 blend, with the criteria of
-test_gpu_blend_edges.run_case (every walk, n_contrib exact, each value inside its derived budget).  Depth is where the
+test_gpu_blend_edges.run_case (n_contrib exact, each value inside its derived budget).  Depth is where the
 kernels' batch logic runs: many 256-entry TMA batches (the forward's double buffer and its mbarrier phases, the
 backward's back-to-front walk that starts with the partial batch), every size class of the tile sort and the global radix
 sort beyond 8192 entries, stops in late batches, and tile_max_contrib cutting a list beyond 512.
@@ -161,7 +161,7 @@ def _check_lists(st, W, H):
         assert np.array_equal(keys[s:e], (np.uint64(tile) << np.uint64(32)) | dbits[want].astype(np.uint64)), (tile, "keys")
 
 
-def _run(name, d, variant, monkeypatch, walls=()):
+def _run(name, d, variant, walls=()):
     """tune the opacities from a first render, then run_case; check the lists, the exclusions and the budget's bars"""
     hier, do_depth = VARIANTS[variant]
     cam = d.sc.cam
@@ -170,9 +170,9 @@ def _run(name, d, variant, monkeypatch, walls=()):
     _check_lists(st0, cam.W, cam.H)          # the walls are placed by list position
     op = _opacities(d, st0, walls)
     assert op.max() <= WALL_ALPHA * 1.001
-    ref, rec, runs = run_case(f"{name} {variant}", d.sc, monkeypatch, hier=hier, do_depth=do_depth, op=op, seed=11,
-                              max_near_pixels=0.0, max_near_gauss=0.0)
-    st = runs[0][2]
+    ref, rec, run = run_case(f"{name} {variant}", d.sc, hier=hier, do_depth=do_depth, op=op, seed=11,
+                             max_near_pixels=0.0, max_near_gauss=0.0)
+    st = run[2]
     _check_lists(st, cam.W, cam.H)
     assert np.array_equal(st["point_list"], st0["point_list"])
     # the construction holds: no pixel near a decision, (nearly) every listed Gaussian compared
@@ -192,7 +192,7 @@ def _run(name, d, variant, monkeypatch, walls=()):
     print(f"[{name} {variant}] lists up to {lens.max()} entries, {compared:.1%} of {listed.size} listed Gaussians "
           f"compared, up to {int(ref['npix'].max())} pixels per Gaussian; median budget / value: colour {col_rel:.2e}, "
           f"sums {acc_rel:.2e}")
-    return ref, runs, lens
+    return ref, run, lens
 
 
 def _fill_tile(d, tx, ty, n, depths, rng):
@@ -204,7 +204,7 @@ def _fill_tile(d, tx, ty, n, depths, rng):
 
 # ---- every size class of the tile sort and every batch boundary ----------------------------------------------------------
 @pytest.mark.parametrize("variant", list(VARIANTS))
-def test_every_sort_class_and_batch_boundary(variant, monkeypatch):
+def test_every_sort_class_and_batch_boundary(variant):
     """One 160 x 64 frame whose tiles hold 1, 128, 129, 256, 257, 511, 512, 513, 1024, 1025, 2048, 4097 and 8192
     entries: every register-sort class and the shared-memory network of the tile sort, and 1 to 32 TMA batches.  The deep
     tiles also lie under medium Gaussians (sigma 4 to 12 px) whose sums collect thousands of pixels.  Depths come from 40
@@ -226,20 +226,20 @@ def test_every_sort_class_and_batch_boundary(variant, monkeypatch):
     for n, (tx, ty) in place.items():
         assert n >= under(tx, ty)
         _fill_tile(d, tx, ty, n - under(tx, ty), depths, rng)
-    ref, runs, lens = _run("sort classes", d, variant, monkeypatch)
+    ref, run, lens = _run("sort classes", d, variant)
     for n, (tx, ty) in place.items():
         assert lens[ty * gx + tx] == n, (n, int(lens[ty * gx + tx]))
     assert lens.max() == 8192
     # Gaussians whose sums collect thousands of pixels, pixels that take hundreds of entries
     assert ref["npix"].max() > 1000
     assert ref["n_contrib"].max() > 4 * BATCH
-    dep = runs[0][2]["depths"][runs[0][2]["radii"] > 0]
+    dep = run[2]["depths"][run[2]["radii"] > 0]
     assert np.unique(dep).size <= 40 < dep.size
 
 
 # ---- the global radix sort beyond 8192 entries ---------------------------------------------------------------------------
 @pytest.mark.parametrize("variant", list(VARIANTS))
-def test_radix_sort_hand_over(variant, monkeypatch):
+def test_radix_sort_hand_over(variant):
     """A tile of 8200 entries, beyond the shared-memory sort: the whole frame is binned by the global radix sort, whose
     stable order over (tile, depth) must equal the per-tile sort's (depth, index)."""
     d = Deep(48, 32, VARIANTS[variant][0], seed=41)
@@ -247,7 +247,7 @@ def test_radix_sort_hand_over(variant, monkeypatch):
     depths = 2.0 + 0.05 * np.arange(30)
     for (tx, ty), n in (((1, 0), RADIX), ((0, 1), 300), ((2, 1), 1), ((0, 0), 129)):
         _fill_tile(d, tx, ty, n, depths, rng)
-    ref, runs, lens = _run("radix", d, variant, monkeypatch)
+    ref, run, lens = _run("radix", d, variant)
     assert lens.max() == RADIX and sorted(lens[lens > 0]) == [1, 129, 300, RADIX]
     assert ref["n_contrib"].max() > 16 * BATCH
 
@@ -292,7 +292,7 @@ def _wall_sequence(n, walls, last, rng):
 
 
 @pytest.mark.parametrize("variant", list(VARIANTS))
-def test_walls_at_batch_edges_and_cuts(variant, monkeypatch):
+def test_walls_at_batch_edges_and_cuts(variant):
     """Walls at 1-based list positions 256k - 1, 256k and 256k + 1 (k = 1..4) and at the last entry, each in another
     8x8 quadrant of its tile, so that warps and groups of one tile stop in different batches; the pixels without a wall
     never stop.  In the last five tiles nothing behind entry 512, 513, 700, 1024 or 1025 is taken by any pixel, so
@@ -310,8 +310,8 @@ def test_walls_at_batch_edges_and_cuts(variant, monkeypatch):
                 o = opac[role] if role != "bg" else (0.009 if rng.uniform() < 1 / 3 else 0.045)
                 d.add(TILE * (t % gx) + a, TILE * (t // gx) + b, 2.0 + 0.004 * (j // 3), TINY, o, role)
     walls = [(t, p, TILE * (t % gx) + a, TILE * (t // gx) + b) for t, (_, ws, _) in enumerate(WALL_TILES) for p, (a, b) in ws]
-    ref, runs, lens = _run("walls", d, variant, monkeypatch, walls=walls)
-    st = runs[0][2]
+    ref, run, lens = _run("walls", d, variant, walls=walls)
+    st = run[2]
     assert [int(lens[t]) for t in range(len(WALL_TILES))] == [n for n, _, _ in WALL_TILES]
     positions = sorted(p for _, p, _, _ in walls)
     assert {256 * k + e for k in range(1, 5) for e in (-1, 0, 1)} <= set(positions)

@@ -10,8 +10,6 @@ phases=1)).  Then, outside the pixels that have a pair within the decision margi
     rcp.approx + one Newton step ~1 ulp, the exponent's ulps on the magnitude of its terms, the hierarchy weight's
     branches <= 4e-6, the transmittance's error accumulated along the pixel's list) times the pair's absolute term,
     plus n U times the absolute-sum scale for the n-term fp32 sum (blend_ref.py states the derivation term by term).
-Each case runs under both walks of each kernel (H3DGS_GROUPWALK unset, 0 and 1): the forward outputs must be
-bit-identical across the walks, the sums equal up to the order of their fp32 additions.
 
 The measured maxima of |kernel - float64| / budget are printed per case (run with -s); each must stay <= 1."""
 import math
@@ -23,7 +21,6 @@ from blend_ref import blend_reference, compare, hier_weight, ALPHA_CAP, ALPHA_SK
 
 pytestmark = pytest.mark.gpu
 
-WALKS = (None, "0", "1")
 FOVX = 60.0
 
 
@@ -95,22 +92,15 @@ def _grads(cam, seed):
     return (g.standard_normal((3, cam.H, cam.W)) / 64).astype(np.float32), (g.standard_normal((cam.H, cam.W)) / 64).astype(np.float32)
 
 
-def run_case(name, sc, monkeypatch, hier=False, do_depth=False, bg=(0.1, 0.4, 0.9), op=None, seed=0,
+def run_case(name, sc, hier=False, do_depth=False, bg=(0.1, 0.4, 0.9), op=None, seed=0,
              max_near_pixels=1e-3, max_near_gauss=0.05):
-    """Render `sc` under the three walks; check each against blend_ref and the walks against each other.
-    Returns (reference dict, records, list of (color, invdepth, state, accum) per walk)."""
+    """Render `sc` and check it against blend_ref.
+    Returns (reference dict, records, (color, invdepth, state, accum))."""
     cam = sc.cam
     bg = np.asarray(bg, np.float32)
     gcol, gdep = _grads(cam, seed)
-    runs = []
-    for walk in WALKS:
-        if walk is None:
-            monkeypatch.delenv("H3DGS_GROUPWALK", raising=False)
-        else:
-            monkeypatch.setenv("H3DGS_GROUPWALK", walk)
-        runs.append(_render(sc, bg, hier, do_depth, gcol, gdep, op))
-    monkeypatch.delenv("H3DGS_GROUPWALK", raising=False)
-    color, invd, st, accum = runs[0]
+    run = _render(sc, bg, hier, do_depth, gcol, gdep, op)
+    color, invd, st, accum = run
     vis = st["radii"] > 0
     rec = st["records"].copy()
     rec[~vis] = 0                      # rows K1 did not write (culled) are never listed
@@ -127,37 +117,25 @@ def run_case(name, sc, monkeypatch, hier=False, do_depth=False, bg=(0.1, 0.4, 0.
     assert gshare <= max_near_gauss, (name, gshare, ref["near_kind"])
     rows = ~ref["near_gauss"]
     report = {}
-    for w, (c_, i_, s_, a_) in zip(WALKS, runs):
-        assert np.array_equal(s_["records"][vis].view(np.uint32), st["records"][vis].view(np.uint32))
-        nc = s_["n_contrib"].astype(np.int64)
-        bad = (nc != ref["n_contrib"]) & keep
-        assert not bad.any(), (name, w, "n_contrib", int(bad.sum()), np.argwhere(bad)[:5].tolist())
-        checks = [("color", c_, ref["color"], ref["color_tol"][None], keep[None]),
-                  ("final_T", s_["final_T"], ref["final_T"], ref["final_T_tol"], keep)]
-        if do_depth:
-            checks.append(("invdepth", i_, ref["invdepth"], ref["invdepth_tol"], keep))
-        cols = list(range(9)) + ([9] if do_depth else [])
-        for c in cols:
-            checks.append((f"accum[{c}]", a_[:, c], ref["accum"][:, c], ref["accum_tol"][:, c], rows))
-        for what, got, want, tol, mask in checks:
-            r, cnt = compare(got, want, tol, mask)
-            report[what] = max(report.get(what, 0.0), r)
-            assert r <= 1.0, (name, w, what, r)
-        if not do_depth:
-            assert np.all(a_[:, 9] == 0)
-    # the walks: forward bit for bit, the sums up to the order of their additions
-    for c_, i_, s_, a_ in runs[1:]:
-        assert np.array_equal(c_.view(np.uint32), color.view(np.uint32))
-        assert np.array_equal(s_["final_T"].view(np.uint32), st["final_T"].view(np.uint32))
-        assert np.array_equal(s_["n_contrib"], st["n_contrib"])
-        if do_depth:
-            assert np.array_equal(i_.view(np.uint32), invd.view(np.uint32))
-        d = np.abs(a_.astype(np.float64) - accum)
-        lim = 2 * (8 + ref["npix"])[:, None] * U * ref["accum_abs"] + 1e-30
-        assert (d <= lim).all(), (name, "walks", float((d / lim).max()))
+    nc = st["n_contrib"].astype(np.int64)
+    bad = (nc != ref["n_contrib"]) & keep
+    assert not bad.any(), (name, "n_contrib", int(bad.sum()), np.argwhere(bad)[:5].tolist())
+    checks = [("color", color, ref["color"], ref["color_tol"][None], keep[None]),
+              ("final_T", st["final_T"], ref["final_T"], ref["final_T_tol"], keep)]
+    if do_depth:
+        checks.append(("invdepth", invd, ref["invdepth"], ref["invdepth_tol"], keep))
+    cols = list(range(9)) + ([9] if do_depth else [])
+    for c in cols:
+        checks.append((f"accum[{c}]", accum[:, c], ref["accum"][:, c], ref["accum_tol"][:, c], rows))
+    for what, got, want, tol, mask in checks:
+        r, cnt = compare(got, want, tol, mask)
+        report[what] = r
+        assert r <= 1.0, (name, what, r)
+    if not do_depth:
+        assert np.all(accum[:, 9] == 0)
     print(f"\n[{name}] max |kernel - f64| / budget: " + " ".join(f"{k}={v:.3g}" for k, v in report.items()) +
           f"  excluded: {near_share:.2e} of pixels, {gshare:.2e} of Gaussians {ref['near_kind']}")
-    return ref, rec, runs
+    return ref, rec, run
 
 
 def _gauss_at(rec, i, u, v):
@@ -185,7 +163,7 @@ SWEEP_KIDS = [0, 1, 2, 3, 4, 7, 16, 17, 64, 255, 1000, 4095, 4096, 4097, 65535, 
 
 @pytest.mark.parametrize("t", [0.0, 2.0 ** -24, 0.5, 1.0 - 2.0 ** -24, 1.0])
 @pytest.mark.parametrize("do_depth", [False, True])
-def test_hierarchy_weight_sweep(t, do_depth, monkeypatch):
+def test_hierarchy_weight_sweep(t, do_depth):
     """One 6-row band per num_node_kids value; in each, two long Gaussians (from the left and the right edge, slightly
     different widths so their alphas interleave) whose base alpha falls from the 0.99 cap to below 1/255 across the
     image: every band crosses alpha = 1/16 (the series / MUFU switch) and the 1/255 cut many times."""
@@ -196,7 +174,7 @@ def test_hierarchy_weight_sweep(t, do_depth, monkeypatch):
         v = 6 * b + 2.5
         sc.add(0, v, 3.0 + 0.01 * b, 45.0, 2.5, op=1.2, t=t, k=k, rng=rng)
         sc.add(cam.W - 1, v + 0.5, 4.0 + 0.01 * b, 47.3, 2.3, op=1.1, t=t, k=k, rng=rng)
-    ref, rec, runs = run_case(f"sweep t={t:.9g} depth={do_depth}", sc, monkeypatch, hier=True, do_depth=do_depth, seed=2)
+    ref, rec, run = run_case(f"sweep t={t:.9g} depth={do_depth}", sc, hier=True, do_depth=do_depth, seed=2)
     # the bands do blend where they should: the identity counts everywhere, the others as far as their weight allows
     nc = ref["n_contrib"]
     assert (nc > 0).mean() > 0.5
@@ -207,7 +185,7 @@ def test_hierarchy_weight_sweep(t, do_depth, monkeypatch):
         own = lambda band: ref["accum"][2 * band:2 * band + 2, 6:9]
         assert np.abs(own(two)).sum() > 0
         if t == 0.0:
-            assert np.all(own(b) == 0) and np.all(runs[0][3][2 * b:2 * b + 2] == 0)
+            assert np.all(own(b) == 0) and np.all(run[3][2 * b:2 * b + 2] == 0)
 
 
 # ---- the alpha = 1/255 cut ---------------------------------------------------------------------------------------------
@@ -215,7 +193,7 @@ SKIP_MODES = [(1.0, 1), (0.3, 2), (0.0, 7), (0.0, 300), (0.5, 40)]
 
 
 @pytest.mark.parametrize("hier", [False, True])
-def test_skip_threshold_both_sides(hier, monkeypatch):
+def test_skip_threshold_both_sides(hier):
     """Isolated Gaussians, each tuned so that its alpha (after the hierarchy weight) at one chosen pixel is
     1/255 (1 +- 1e-3): taken on the + side, skipped on the - side."""
     cam = _cam(160, 120)
@@ -236,7 +214,7 @@ def test_skip_threshold_both_sides(hier, monkeypatch):
     for j, u, v, t, k, s in targets:
         a = _base_alpha_for(ALPHA_SKIP * (1 + s * 1e-3), t, k) if hier else ALPHA_SKIP * (1 + s * 1e-3)
         op[j] = a / _gauss_at(st["records"], j, u, v)
-    ref, rec, runs = run_case(f"skip hier={hier}", sc, monkeypatch, hier=hier, op=op, seed=4)
+    ref, rec, run = run_case(f"skip hier={hier}", sc, hier=hier, op=op, seed=4)
     for j, u, v, t, k, s in targets:
         assert not ref["near_pixel"][v, u]
         assert (ref["n_contrib"][v, u] > 0) == (s > 0), (j, t, k, s)          # the scene is what it claims to be
@@ -245,7 +223,7 @@ def test_skip_threshold_both_sides(hier, monkeypatch):
 # ---- the T < 1e-4 stop, at the TMA batch edges -------------------------------------------------------------------------
 @pytest.mark.parametrize("stop_at,n", [(255, 300), (256, 300), (299, 300)])
 @pytest.mark.parametrize("side", [-1, 1])
-def test_stop_threshold_at_batch_edges(stop_at, n, side, monkeypatch):
+def test_stop_threshold_at_batch_edges(stop_at, n, side):
     """A stack of n small Gaussians over one pixel; there the transmittance in front of entry `stop_at` is 2e-4 and that
     entry brings T (1 - alpha) to 1e-4 (1 + side 1e-3): the list stops there (side -1) or goes on (side +1).  stop_at =
     255 / 256 are the last entry of the first 256-entry TMA batch and the first of the second, 299 the last of the list.
@@ -264,17 +242,17 @@ def test_stop_threshold_at_batch_edges(stop_at, n, side, monkeypatch):
     op[:stop_at] = a_front / G[:stop_at]
     Tb = np.prod(1 - np.float32(op[:stop_at]).astype(np.float64) * G[:stop_at])
     op[stop_at] = (1 - T_STOP * (1 + side * 1e-3) / Tb) / G[stop_at]
-    ref, rec, runs = run_case(f"stop at {stop_at}/{n} side {side}", sc, monkeypatch, op=op, seed=6)
+    ref, rec, run = run_case(f"stop at {stop_at}/{n} side {side}", sc, op=op, seed=6)
     assert not ref["near_pixel"][v0, u0]
     if side < 0:
         assert ref["n_contrib"][v0, u0] == stop_at                 # entry stop_at (0-based) ends the list, unblended
     else:
         assert ref["n_contrib"][v0, u0] == stop_at + 1             # blended; the next entry (alpha 0.3) stops
-    assert runs[0][2]["n_contrib"][v0, u0] == ref["n_contrib"][v0, u0]
+    assert run[2]["n_contrib"][v0, u0] == ref["n_contrib"][v0, u0]
 
 
 # ---- the 0.99 cap, opacity above 1 -------------------------------------------------------------------------------------
-def test_alpha_cap_both_sides(monkeypatch):
+def test_alpha_cap_both_sides():
     """Isolated Gaussians with opacity above 1 whose opacity G at one pixel is 0.99 (1 +- 1e-3).  The cap is not
     differentiated (the published backward): above it the pixel still passes G dL/dalpha to the opacity, continuous
     across the cap -- so blend_ref and the kernel must agree on both sides, and the capped pixels' sums are not 0."""
@@ -292,16 +270,16 @@ def test_alpha_cap_both_sides(monkeypatch):
     for j, u, v, s in targets:
         op[j] = ALPHA_CAP * (1 + s * 1e-3) / _gauss_at(st["records"], j, u, v)
     assert op.min() > 1.0
-    ref, rec, runs = run_case("cap", sc, monkeypatch, op=op, seed=8)
+    ref, rec, run = run_case("cap", sc, op=op, seed=8)
     for j, u, v, s in targets:
         assert not ref["near_pixel"][v, u] and ref["n_contrib"][v, u] > 0
-        assert runs[0][3][j, 5] != 0 and ref["accum"][j, 5] != 0
+        assert run[3][j, 5] != 0 and ref["accum"][j, 5] != 0
 
 
 # ---- image borders, tiny images, off-screen means, needles -------------------------------------------------------------
 @pytest.mark.parametrize("W,H", [(13, 9), (64, 47), (160, 119)])
 @pytest.mark.parametrize("hier", [False, True])
-def test_borders_offscreen_and_needles(W, H, hier, monkeypatch):
+def test_borders_offscreen_and_needles(W, H, hier):
     """Odd H (the second pixel of a thread outside the image), images below one tile, Gaussians centred off screen
     (the 1.3 tan(fov) clamp of the projection is active), and thin needle-shaped conics centred in a 4x4 block, so that
     their reach mask covers only a few of the tile's blocks."""
@@ -325,9 +303,9 @@ def test_borders_offscreen_and_needles(W, H, hier, monkeypatch):
         else:                  # ordinary, some large
             sc.add(rng.uniform(-3, W + 3), rng.uniform(-3, H + 3), z, rng.uniform(0.5, 6), rng.uniform(0.5, 6),
                    rho=rng.uniform(-0.8, 0.8), op=rng.uniform(0.05, 1.2), t=t, k=k, rng=rng)
-    ref, rec, runs = run_case(f"borders {W}x{H} hier={hier}", sc, monkeypatch, hier=hier, do_depth=hier, seed=9,
-                              max_near_gauss=0.1)
-    st = runs[0][2]
+    ref, rec, run = run_case(f"borders {W}x{H} hier={hier}", sc, hier=hier, do_depth=hier, seed=9,
+                             max_near_gauss=0.1)
+    st = run[2]
     assert (ref["n_contrib"] > 0).mean() > 0.5
     # the clamp is active for some visible off-screen means
     xv = np.array(sc.means)[:, 0] / np.array(sc.means)[:, 2]

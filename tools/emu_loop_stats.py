@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Development aid (CPU, emulation build): loop statistics of the blend kernels on a 1/16-scale config #3 frame --
-warp iterations, no-taker exits, pixel-entries actually blended, per-group iterations -- for both walk variants.
+warp iterations, no-taker exits, pixel-entries actually blended, per-group iterations.
 usage: python tools/emu_loop_stats.py [leaves=94000]"""
 import ctypes as C
 import os
@@ -31,16 +31,14 @@ emu = Emu(build(tempfile.mkdtemp(prefix="h3dgs_emu_stats")))
 emu.L.h3dgs_emu_stats.restype = C.POINTER(C.c_longlong)
 st = emu.L.h3dgs_emu_stats()
 bg = np.zeros(3, np.float32)
-for gw in ("0", "1"):
-    os.environ["H3DGS_GROUPWALK"] = gw
-    for i in range(16):
-        st[i] = 0
-    a, keep = emu.args(cam, bg, h, ts=ts, kids=kids, ridx=ri, pidx=pi)
-    fw = emu.forward(a, keep)
-    g = emu.backward(a, fw, synth.l1_grad(fw["color"]))
-    s = [st[i] for i in range(16)]
-    V = int((fw["radii"] > 0).sum())
-    print(f"groupwalk={gw}: cut {n} V {V} D {fw['D']} (D/V {fw['D'] / V:.2f}, mean tile list {fw['D'] / (((W + 15) // 16) * ((H + 15) // 16)):.0f}); t<1 on {float((ts < 1).mean()):.2f} of the cut")
-    print(f"  forward : {s[8]} warp iterations, {s[9]} pixel-entries blended -> {s[9] / max(s[8], 1):.1f} of 64 pixels per iteration; group-iterations {s[10]} ({s[10] / max(s[8], 1):.2f} of 4 per iteration)")
-    print(f"  backward: {s[0]} warp iterations, {s[1]} ({s[1] / max(s[0], 1):.2%}) leave at the no-taker vote, {s[2]} pixel-entries -> {s[2] / max(s[0] - s[1], 1):.1f} of 64 per full iteration; "
-          f"group-iterations {s[3]}, of which {s[4]} without a taker")
+for i in range(16):
+    st[i] = 0
+a, keep = emu.args(cam, bg, h, ts=ts, kids=kids, ridx=ri, pidx=pi)
+fw = emu.forward(a, keep)
+g = emu.backward(a, fw, synth.l1_grad(fw["color"]))
+s = [st[i] for i in range(16)]
+V = int((fw["radii"] > 0).sum())
+print(f"cut {n} V {V} D {fw['D']} (D/V {fw['D'] / V:.2f}, mean tile list {fw['D'] / (((W + 15) // 16) * ((H + 15) // 16)):.0f}); t<1 on {float((ts < 1).mean()):.2f} of the cut")
+print(f"  forward : {s[8]} warp iterations, {s[9]} pixel-entries blended -> {s[9] / max(s[8], 1):.1f} of 64 pixels per iteration")
+print(f"  backward: {s[0]} warp iterations, {s[1]} ({s[1] / max(s[0], 1):.2%}) leave at the no-taker vote, {s[2]} pixel-entries -> {s[2] / max(s[0] - s[1], 1):.1f} of 64 per full iteration; "
+      f"group-iterations {s[3]}, of which {s[4]} without a taker")

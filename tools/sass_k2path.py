@@ -3,7 +3,7 @@
 k = 2 hierarchy path (the innermost loop around the MUFU.RSQ of pair_hier_alpha, minus the general-k block), e.g.
 
   python tools/sass_k2path.py hierarchical-3d-gaussians_b200/build/render_backward.o \\
-      _ZN5h3dgs22render_backward_kernelILb1ELb0ELb1E
+      _ZN5h3dgs22render_backward_kernelILb1ELb0EE
 
 Needs cuobjdump on PATH; no GPU."""
 import re, subprocess, sys, collections
